@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the SceneDreamer per-pixel render hot path on B200 (BASELINE.json metric).
+"""Benchmark of the SceneDreamer per-pixel render hot path on H100 (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W            # our arm (CUDA, libsdb200)
     python bench.py --impl reference --steps K --warmup W    # reference arm: CPU path on host cores
@@ -7,11 +7,11 @@
 A "step" is ONE frame of the C2 workload (BASELINE.md): 540x960 output pixels, 24 samples/ray,
 scene_size 1024, cam_mode 0, pad 30 -> 570x990 rays raycast + shaded:
     a1  ray/voxel DDA                        (sdb_ray_voxel_intersection_perspective_ex, exact empty-space flight)
-    a9  sky branch: PE + SKYMLP + frame mean  (sdb_sky_forward: same tcgen05 engine, per ray)
-    a2-a8, a10-a12 fused per-pixel kernel    (sdb_render_rays_forward: tcgen05 MLP, hash gather, compositing)
-    f1  RenderCNN + tanh (e2e only)          (sdb_cnn_forward: tcgen05 implicit-GEMM convolution over the whole padded frame)
+    a9  sky branch: PE + SKYMLP + frame mean  (sdb_sky_forward: same wgmma engine, per ray)
+    a2-a8, a10-a12 fused per-pixel kernel    (sdb_render_rays_forward: wgmma MLP, hash gather, compositing)
+    f1  RenderCNN + tanh (e2e only)          (sdb_cnn_forward: wgmma implicit-GEMM convolution over the whole padded frame)
 Credit = OUTPUT samples: 518,400 px x 24 = 12,441,600 samples per frame (padding rays are overhead).
-`value` is the per-pixel path a1-a12 with inputs resident (SURVEY.md 8(d)); `e2e` goes from a host pose to the RGB image on
+`value` is the per-pixel path a1-a12 with inputs resident; `e2e` goes from a host pose to the RGB image on
 the host (RenderCNN included).  Both are the product default: the fused kernel runs its rows as RAY SLOTS -- a ray leaves its
 row once its transmittance is < 1e-7 and the next live ray of the frame takes the row; `value_exact_march` is the same
 measurement with that early termination off (every sample of every live ray shaded) -- the two differ by less than 2e-7 in the
@@ -21,7 +21,7 @@ per-step CUDA events).
 Multi-GPU: weak scaling by default (every rank renders its own frames, frame f -> rank f mod N; the finished frames are
 all-gathered once per step over NCCL); `--mode strong` splits ONE frame into 16-row bands dealt round-robin
 to the ranks (one banded raycast and one render launch per rank).
-Extra keys at N=1: `c4` (2160x3840x40), `c5_train_step` (bench_train.py), `reference_cuda_b200` (the reference renderer itself
+Extra keys at N=1: `c4` (2160x3840x40), `c5_train_step` (bench_train.py), `reference_cuda` (the reference renderer itself
 on this GPU, and the same Python with dropin/ on the path), `cpu_baseline`.
 """
 import argparse
@@ -50,7 +50,7 @@ OUT_HW = (540, 960)
 PAD = 30
 SPP = 24
 SCENE = 1024
-BYTES_PER_SAMPLE = 16384 + 344.0 / SPP     # SURVEY.md 8(d): table gather + per-ray I/O
+BYTES_PER_SAMPLE = 16384 + 344.0 / SPP     # BASELINE.md 2b: table gather + per-ray I/O
 SAMPLES_PER_FRAME = OUT_HW[0] * OUT_HW[1] * SPP
 PIX_PER_FRAME = OUT_HW[0] * OUT_HW[1]
 
@@ -59,12 +59,12 @@ def measured_peaks():
     p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(p):
         d = json.load(open(p))
-        return float(d['hbm_gbs']), float(d.get('bf16_tflops_sustained', d.get('bf16_tflops', 1430.0))), 'measured'
-    return 6650.0, 1400.0, 'fallback'
+        return float(d['hbm_gbs']), float(d.get('bf16_tflops_sustained', d.get('bf16_tflops', 989.0))), 'measured'
+    return 3350.0, 989.0, 'H100 SXM data sheet (dense bf16, 700 W)'
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md): one streaming
+    """nvidia-smi clocks / throttle reasons DURING the timed region (sampled while the steps run): one streaming
     `nvidia-smi -lms 100` process, lines collected by this thread."""
 
     QUERY = ('clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,'
@@ -181,7 +181,7 @@ WORKLOADS = {
     'c3': ((540, 960), 24, 1024, 4, 'C3: 40-frame trajectory cam_mode=4, 540x960, num_samples=24, scene_size=1024, frames sharded over the ranks'),
     'c4': ((2160, 3840), 40, 2048, 0, 'C4: single 2160x3840 frame, num_samples=40, scene_size=2048'),
 }
-FLOP_PER_SAMPLE = 754176          # LightningMLP, SURVEY.md 8(a8)
+FLOP_PER_SAMPLE = 754176          # LightningMLP
 
 
 def pin_rank_to_gpu_numa(local):
@@ -327,6 +327,8 @@ def run_gpu_arm(args):
     host_rgb = torch.empty(3, out_hw[0], out_hw[1], dtype=torch.float32).pin_memory()
     e2e_image = not strong                    # the user-facing result of a frame is the IMAGE: RenderCNN + tanh (f1) on top of the path
 
+    last = {}                                 # the most recent step's result maps (for --dump-outputs)
+
     def one_step(k, ev=None, kev=None, cev=None, want_host=True, to_image=False):
         idx = (k if strong else (k * world_size + rank)) % len(cams)
         cam = cams[idx]
@@ -347,6 +349,7 @@ def run_gpu_arm(args):
                 cev[1].record()
             if strong:                                               # slot j of rank r is band j * N + r: back into frame order
                 maps = sharding.assemble_bands(allm, world_size, n_slots, band_cap)
+        last['maps'] = maps
         if want_host:                                                # D2H of the step's result
             if to_image:
                 host_rgb.copy_(maps, non_blocking=True)
@@ -373,11 +376,13 @@ def run_gpu_arm(args):
     launches0 = int(L.sdb_launch_count())
     t_begin = time.perf_counter()
     for k in range(args.steps):
-        one_step(k, evs[k], kevs[k], cevs[k], to_image=e2e_image)
+        last_out = one_step(k, evs[k], kevs[k], cevs[k], to_image=e2e_image)
         torch.cuda.synchronize()                                     # the caller READS the step's result on the host
         flush.zero_()                                                # L2 flush between timed iterations
     torch.cuda.synchronize()
     t_wall = time.perf_counter() - t_begin
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last['maps'], last_out)
     launches = int(L.sdb_launch_count()) - launches0
     if world_size > 1:
         dist.barrier()
@@ -474,7 +479,7 @@ def run_gpu_arm(args):
             'config': {'workload': wl_name + ', pad %d (%dx%d rays cast+shaded, %d px credited); ' % (PAD, res[0], res[1], out_hw[0] * out_hw[1]) +
                                    ('ONE frame per step in 16-row bands dealt round-robin to the GPUs' if strong else 'one frame per GPU per step'),
                        'precision': args.precision, 'l2': 'flushed between steps (256 MiB memset) + a different pose each step',
-                       'table': 'per-scene pre-blended 3-D table (8 corners/level)', 'sky_mlp': 'tcgen05 engine (sdb_sky_forward)',
+                       'table': 'per-scene pre-blended 3-D table (8 corners/level)', 'sky_mlp': 'wgmma engine (sdb_sky_forward)',
                        'early_termination': ('off' if args.no_early_stop else
                                              'a ray leaves its MMA row once its transmittance is < %g (skipped samples carry less than '
                                              'that compositing weight; credited like sky-only rays); --no-early-stop marches everything'
@@ -484,8 +489,8 @@ def run_gpu_arm(args):
                     'd2h_bytes_per_step': int((host_rgb if e2e_image else host_out).numel() * 4), 'ms_per_step': tot_ms / args.steps,
                     'result': 'RGB image [3,%d,%d] fp32' % out_hw if e2e_image else 'depth + opacity maps',
                     'note': ('per step: pose from pinned host memory (by value in the launch arguments) -> DDA -> sky -> fused render -> '
-                             'RenderCNN + tanh on the whole padded frame (tcgen05 implicit GEMM, fp16x3) -> crop -> RGB to pinned host, host '
-                             'waits for it.  `value` is the per-pixel path alone (SURVEY 8(d): a1-a12), e2e goes on to the image, so the two '
+                             'RenderCNN + tanh on the whole padded frame (wgmma implicit GEMM, fp16x3) -> crop -> RGB to pinned host, host '
+                             'waits for it.  `value` is the per-pixel path alone (a1-a12), e2e goes on to the image, so the two '
                              'differ by the RenderCNN time (`rendercnn_ms`)') if e2e_image else
                             'per step: pose (by value) -> DDA -> sky -> fused render of this rank\'s row band -> band maps gathered -> host'},
             'gpu_launches': launches,
@@ -507,8 +512,8 @@ def run_gpu_arm(args):
                          'tile_steps_without_early_termination': (np.ceil(live_tiles / 128.0) if ray_slots else live_tiles) * spp,
                          'hbm': {'algorithmic_bytes_per_launch': samples_per_frame * BYTES_PER_SAMPLE,
                                  'algorithmic_GBps': samples_per_frame * band_frac * BYTES_PER_SAMPLE / kern_s / 1e9, 'peak_GBps': hbm,
-                                 'note': 'SURVEY 8(d) prescribes 16,398 B/sample; the kernel does NOT move them (pre-blended table: 4x fewer '
-                                         'corners, L2-resident gathers): measured DRAM traffic is `traffic`, ~600x lower, so HBM is not the bound'}},
+                                 'note': 'BASELINE.md 2b prescribes 16,398 B/sample; the kernel does NOT move them (pre-blended table: 4x fewer '
+                                         'corners, L2-resident gathers), so this is the algorithmic rate, not a measured DRAM rate'}},
             'cpu_baseline': cpu, 'clocks': clocks, 'wall_s': t_wall,
             'per_rank_ms': {'columns': ['e2e_step', 'dda_sky', 'fused_kernel_window', 'collective_incl_wait', 'e2e_step_max', 'cpus_in_affinity'],
                             'rows': table},
@@ -522,9 +527,26 @@ def run_gpu_arm(args):
         dist.destroy_process_group()
 
 
+def dump_outputs(dirname, maps, out):
+    """What the last timed step computed, as float32 .npy files: the step's result maps (the RGB image, or depth and total
+    weight in strong mode), depth and total weight of every ray, and the per-pixel features of a fixed, seeded sample of
+    65,536 rays (all of them would be 144 MB at C2)."""
+    os.makedirs(dirname, exist_ok=True)
+
+    def save(name, t):
+        np.save(os.path.join(dirname, name + '.npy'), t.detach().float().cpu().numpy())
+    save('maps', maps)
+    save('depth', out['depth'])
+    save('total_weight', out['total_weight'])
+    feat = out['net_out'].reshape(-1, out['net_out'].shape[-1])
+    idx = np.sort(np.random.default_rng(0).choice(feat.shape[0], size=min(65536, feat.shape[0]), replace=False))
+    save('net_out_sample', feat[torch.from_numpy(idx).to(feat.device)])
+    np.save(os.path.join(dirname, 'net_out_sample_rows.npy'), idx.astype(np.float64))
+
+
 def extra_legs(args):
     """Reported next to the headline at N=1 (each in a subprocess, bounded): C4 throughput, the C5 train step, and the
-    reference renderer itself on this B200 (its own CUDA extensions + PyTorch, through the real Generator)."""
+    reference renderer itself on this GPU (its own CUDA extensions + PyTorch, through the real Generator)."""
     ex = {}
 
     def run(cmd, timeout):
@@ -562,16 +584,16 @@ def extra_legs(args):
             d = _np.load(out)
             res[backend] = (float(_np.mean(d['perpix_ms'])), float(_np.mean(d['cnn_ms'])))
         spf = SAMPLES_PER_FRAME
-        ex['reference_cuda_b200'] = {
+        ex['reference_cuda'] = {
             'what': "the reference's own Generator.inference_givenstyle (unmodified Python staged in oracle/_ref/py) on this GPU: "
-                    "'reference' = its own CUDA extensions compiled for sm_100a + cuBLAS/ATen, unfused 40-tile loop; 'dropin_zero_edit' = the "
+                    "'reference' = its own CUDA extensions compiled for sm_90a + cuBLAS/ATen, unfused 40-tile loop; 'dropin_zero_edit' = the "
                     'same Python with dropin/ on the path (class-level fused hook, one launch per frame). GPU-timeline ms per C2 frame, '
                     'per-pixel path (raycast + sky pre-pass + _forward_perpix) and RenderCNN (_forward_global) separately',
             'reference': {'perpix_ms': res['ref'][0], 'cnn_ms': res['ref'][1], 'msamples_per_s': spf / (res['ref'][0] * 1e-3) / 1e6},
             'dropin_zero_edit': {'perpix_ms': res['dropin'][0], 'cnn_ms': res['dropin'][1], 'msamples_per_s': spf / (res['dropin'][0] * 1e-3) / 1e6},
             'perpix_speedup': res['ref'][0] / res['dropin'][0]}
     except Exception as e:          # noqa: BLE001
-        ex['reference_cuda_b200'] = {'error': repr(e)[:300]}
+        ex['reference_cuda'] = {'error': repr(e)[:300]}
     return ex
 
 
@@ -587,9 +609,13 @@ def main():
                     help='weak: one frame per GPU per step (frames sharded); strong: ONE frame per step split into row bands')
     ap.add_argument('--no-cpu', action='store_true', help='skip the cpu_baseline leg')
     ap.add_argument('--no-extras', action='store_true', help='skip the C4 / C5 / reference-CUDA legs reported next to the headline at N=1')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last one computed to DIR/<name>.npy (float32, < 64 MB)')
     ap.add_argument('--no-early-stop', action='store_true',
                     help='march every sample of every live tile (early termination off; the reference arithmetic sample for sample)')
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != 'ours' or args.steps < 1):
+        ap.error('--dump-outputs writes what the last timed step of the GPU arm computed: it needs --impl ours and --steps >= 1')
     if args.impl == 'reference':
         run_reference_arm(args)
         return

@@ -2,8 +2,8 @@
 """Train-step benchmark of the per-pixel path (BASELINE.json config 5, per-GPU share): one 256x256 view
 (+6 px pad -> 262x262 rays), 24 samples/ray, scene_size 1024, stratified sampling; renderer forward WITH
 the training record + full backward (all parameter gradients of hash table, scene code, LightningMLP,
-style code, sky net).  Not the headline metric (bench.py is); this is the measurement for SURVEY.md
-section 8 row a7 / config C5.
+style code, sky net).  Not the headline metric (bench.py is); this is the measurement for row a7 /
+config C5 (BASELINE.md).
 
     python bench_train.py [--steps K] [--warmup W] [--no-composition]
 

@@ -1,7 +1,7 @@
 """Import-time stand-in for the StyleGAN2 `upfirdn2d_cuda` extension.
 
 `imaginaire.layers` hard-imports it (imaginaire/third_party/upfirdn2d/upfirdn2d.py:17) although no
-SceneDreamer generator, trainer or config ever executes it (SURVEY.md section 8b).  With dropin/ on
+SceneDreamer generator, trainer or config ever executes it.  With dropin/ on
 PYTHONPATH the import resolves; any attempt to CALL into it fails loudly."""
 
 

@@ -4,7 +4,7 @@ The reference imports it as `import voxlib` / `from voxlib import ray_voxel_inte
 (imaginaire/model_utils/gancraft/voxlib/{__init__,positional_encoding,sp_trilinear}.py) and the
 pybind table it expects is imaginaire/model_utils/gancraft/voxlib/voxlib.cpp:25-31.  Put this
 directory (dropin/) on PYTHONPATH ahead of any built reference extension and the reference's
-Python runs unchanged on the B200-native kernels of libsdb200 (scenedreamer_b200.ops).
+Python runs unchanged on the H100-native kernels of libsdb200 (scenedreamer_b200.ops).
 
 Importing this module also arms the fused per-pixel path: `imaginaire.generators.scenedreamer.Generator`
 is patched at class level as soon as it exists (scenedreamer_b200.integration; SDB200_FUSED=0 turns that off),

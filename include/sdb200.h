@@ -1,5 +1,5 @@
 /*
- * sdb200.h -- C ABI of libsdb200.so, the B200-native (sm_100a) implementation of the
+ * sdb200.h -- C ABI of libsdb200.so, the H100-native (sm_90a) implementation of the
  * SceneDreamer per-pixel render hot path.
  *
  * Conventions
@@ -32,7 +32,7 @@ extern "C" {
 
 /* Library / build information.  Safe to call without a GPU. */
 int sdb_version(void);                 /* 10000*major + 100*minor + patch                 */
-const char *sdb_build_info(void);      /* "sm_100a nvcc X.Y ..." -- static string          */
+const char *sdb_build_info(void);      /* "sm_90a nvcc X.Y ..." -- static string          */
 const char *sdb_error_string(int code);/* cudaGetErrorString for >0, own text for <0      */
 
 /* --------------------------------------------------------------------------------------------
@@ -153,11 +153,15 @@ int sdb_sp_trilinear_worldcoord_backward(const float *d_out_grad, int64_t M, int
 
 /* --------------------------------------------------------------------------------------------
  * a2-a5, a8, a10-a12. Fused per-pixel render: sampling -> labels -> hash-grid features ->
- * style-modulated sigma/colour MLP (tcgen05 tensor cores) -> front-to-back compositing + sky
+ * style-modulated sigma/colour MLP (wgmma tensor cores) -> front-to-back compositing + sky
  * blend.  Replaces the body of Generator._forward_perpix and the tile loop around it
  *   (imaginaire/generators/scenedreamer.py:285-428, :600-628; mc_utils.py:82-161;
  *    model_utils/layers.py:92-126, :241-271; gridencoder.cu:75-224).
  * See sdb_render_params below and DESIGN.md for layouts.
+ * The fused kernels (render, sky, training forward and gradient chains) keep their fp32 layer
+ * accumulators in a library-owned device buffer per (device, stream), allocated on the first
+ * launch that needs it: under CUDA-graph capture such a launch returns SDB_EUNSUPPORTED, so run
+ * one launch of the same size on the stream before capturing.
  * ------------------------------------------------------------------------------------------ */
 typedef struct sdb_render_params {
     /* rays (outputs of a1): n_img images of H x W rays, R = n_img*H*W, row-major like the reference */
@@ -224,7 +228,7 @@ int sdb_render_rays_forward(const sdb_render_params *p, void *stream);
 
 /* Per-scene collapse of the two constant encoder dimensions (inference only):
  * table3[l][i] = sum_j w_j(l) * table[l][i ^ K_j(l)], j over the 4 (dim3,dim4) corners.
- * d_table [L*T, 8] -> d_table3 [L*T, 8].  (SURVEY.md section 8d, "parity-preserving work
+ * d_table [L*T, 8] -> d_table3 [L*T, 8].  (DESIGN.md section 2, "parity-preserving work
  * reductions"; valid because every level is hashed and T is a power of two.)
  * d_global_enc: 2 floats on the device.                                                       */
 int sdb_preblend_table(const float *d_table, float *d_table3, int32_t L, int32_t log2_T, float level_S,
@@ -268,12 +272,12 @@ int sdb_sky_forward(const float *d_raydirs, int32_t n_img, int32_t H, int32_t W,
  * kernel_input_backward gridencoder.cu:227-343 for the table and the scene code):
  *   1. compositing backward (volum_rendering_relu, clamp, sky blend; mc_utils.py:154-161,
  *      scenedreamer.py:373-413)                       -> dL/dc, dL/dsigma per sample, dL/dsky;
- *   2. the data-gradient chain of LightningMLP on the tcgen05 engine (transposed weights, bf16x3)
+ *   2. the data-gradient chain of LightningMLP on the wgmma engine (transposed weights, bf16x3)
  *      -> dZ of every layer (bf16 record) and dL/d features;
  *   3. table backward through the pre-blended 3-D table (vector red.add), un-blend to the raw 5-D
  *      table, and the scene-code gradient;
- *   4. weight gradients: dZ^T * A over all samples on the tensor cores (hand-written tcgen05 kernel: the
- *      bf16 records are MMA-ready tiles, fp32 accumulators in TMEM; csrc/wgrad.cu).
+ *   4. weight gradients: dZ^T * A over all samples on the tensor cores (hand-written wgmma kernel: the
+ *      bf16 records are MMA-ready tiles, fp32 accumulators in registers; csrc/wgrad.cu).
  * The same sdb_render_params as the forward call must be passed (same rays, uniforms, packs).
  * The call is fully asynchronous: the live-tile count of the recorded pass stays on the device (record
  * header), every kernel is launched over the record's capacity and reads it there.
@@ -328,7 +332,7 @@ int sdb_sky_backward(int32_t n_img, int32_t H, int32_t W, const void *d_record, 
                      void *d_workspace, void *stream);
 
 /* --------------------------------------------------------------------------------------------
- * f1 (SURVEY.md 8(f)-1). RenderCNN + tanh on the tensor cores: per-pixel feature map -> image.
+ * f1. RenderCNN + tanh on the tensor cores: per-pixel feature map -> image.
  * Replaces Base3DGenerator._forward_global = RenderCNN.forward + tanh
  *   (imaginaire/generators/gancraft_base.py:172-225, :588-603) for the WHOLE padded frame at once
  *   (the reference's tile loop, scenedreamer.py:600-628, computes the same function tile by tile).
@@ -368,7 +372,7 @@ int sdb_modulate_backward(const void *const d_params[25], void *const d_grads[25
                           float *d_dz, void *stream);
 
 /* --------------------------------------------------------------------------------------------
- * f2 (SURVEY.md 8(f)-2). The Adam step of the hash table in one pass over (param, grad, exp_avg,
+ * f2. The Adam step of the hash table in one pass over (param, grad, exp_avg,
  * exp_avg_sq) -- torch.optim.Adam's arithmetic and state (imaginaire/utils/trainer.py:297-323,
  * configs/scenedreamer_train.yaml:36-61: betas (0, 0.999), eps 1e-7, no weight decay / amsgrad).
  * n elements (multiple of 4, 16-byte aligned arrays); step = count AFTER the increment (>= 1); the
@@ -381,7 +385,7 @@ int sdb_adam_step(float *d_param, const float *d_grad, float *d_exp_avg, float *
                   double beta1, double beta2, double eps, int64_t step, void *stream);
 
 /* --------------------------------------------------------------------------------------------
- * f4 (SURVEY.md 8(f)-4). Rejection statistics of the training camera sampler, one pass on the
+ * f4. Rejection statistics of the training camera sampler, one pass on the
  * device (Generator._get_batch, imaginaire/generators/scenedreamer.py:127-142):
  *   d_stats[0] = mean of the non-NaN first-hit entry depths depth2[0, :, :, 0]
  *   d_stats[1] = -sum_k p_k log(p_k + 1e-10), p_k = share of rays whose first voxel id is k (n_bins = 680)
@@ -392,7 +396,7 @@ int sdb_pose_stats(const int32_t *d_voxel_id, const float *d_depth2, int32_t H, 
                    float *d_stats, void *d_workspace, void *stream);
 
 /* --------------------------------------------------------------------------------------------
- * f3 (SURVEY.md 8(f)-3). Voxel world of a scene from its bird's-eye-view maps, built in HBM.
+ * f3. Voxel world of a scene from its bird's-eye-view maps, built in HBM.
  * Replaces the CPU scatter passes, the per-tree Python loop and the 1-4 GB host->device copy of
  * PCGVoxelGenerator.next_world (imaginaire/model_utils/pcg_gen.py:83-174).
  *   sdb_world_build: d_hq / d_label int32 [X, Z] (quantised height index, block id per column);
@@ -417,7 +421,7 @@ int sdb_debug_train_layout(int32_t n_img, int32_t H, int32_t W, int32_t S, int32
  * kernels (role, step, layer markers); pass NULL to disable (default).                          */
 void sdb_debug_set_progress_buffer(void *mapped);
 
-/* tcgen05 / TMEM self test: C[128,N] = A[128,K] * B[N,K]^T with the exact smem descriptors the
+/* tensor-core (wgmma) self test: C[128,N] = A[128,K] * B[N,K]^T with the exact smem descriptors the
  * fused kernel uses.  d_a, d_b fp32 inputs (rounded to fp16/bf16 inside), d_c fp32 output.
  * variant 0 = the layout the library uses; 1 = LBO/SBO swapped (diagnostic only).              */
 int sdb_tc_selftest(const float *d_a, const float *d_b, float *d_c, int32_t N, int32_t K,

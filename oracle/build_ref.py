@@ -1,8 +1,8 @@
 """Build the UNMODIFIED reference CUDA extensions into oracle/_ref/ (test infrastructure only).
 
-The sources are compiled where they lie under /root/reference (nothing is copied into this
-repo); outputs go only to oracle/_ref/, which is git-ignored but travels to the GPU box.
-Two torch extensions are produced for sm_100a:
+The sources are compiled where they lie (SD_REFERENCE_ROOT; nothing is copied into this repo);
+outputs go only to oracle/_ref/, which is git-ignored.
+Two torch extensions are produced for sm_90a:
 
   oracle/_ref/ref_voxlib/ref_voxlib.so            <- imaginaire/model_utils/gancraft/voxlib/*.{cpp,cu}
   oracle/_ref/ref_gridencoder/ref_gridencoder.so  <- gridencoder/src/{gridencoder.cu,bindings.cpp}
@@ -12,12 +12,12 @@ and the reference's own Python (the `imaginaire` and `gridencoder` packages, `en
 
   oracle/_ref/py/                                 <- *.py / *.yaml only (about 1 MB)
 
-so that the GPU box -- where /root/reference does not exist -- can import the real
-`imaginaire.generators.scenedreamer.Generator` (oracle/refgen.py).  oracle/_ref/ is git-ignored: nothing of the
-reference enters this repository's history; it travels with the gpurun snapshot like the built .so files.
+so that a GPU machine without the reference's sources can import the real
+`imaginaire.generators.scenedreamer.Generator` (oracle/refgen.py) when oracle/_ref/ is copied there with the tree.
+oracle/_ref/ is git-ignored: nothing of the reference enters this repository's history.
 
-They are used ONLY by tests and by the "reference CUDA on B200" baseline leg of bench.py as the thing we compare
-against, never by the product path.  Skips silently when /root/reference is absent (the GPU box uses the prebuilt files).
+They are used ONLY by tests and by the "reference CUDA" baseline leg of bench.py as the thing we compare
+against, never by the product path.  Skips silently when the reference's sources are absent (prebuilt files, if any, are used).
 """
 import os
 import sys
@@ -54,7 +54,7 @@ def build(verbose=False):
         print("[oracle/build_ref] %s absent: nothing to build" % REF)
         return False
     stage_python()
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0a")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     os.environ.setdefault("MAX_JOBS", "4")
     from torch.utils.cpp_extension import load
     vox = os.path.join(REF, "imaginaire/model_utils/gancraft/voxlib")

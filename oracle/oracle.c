@@ -59,7 +59,7 @@ void sdo_camera_frame(const float *cam_dir, const float *cam_up, float *fwd, flo
  *   out_depth    [2, H, W, M]   float   (entry t, exit t; NaN when the slot is unfilled)
  *   out_raydirs  [H, W, 3]      float
  * steps_out (optional, [H,W] int32) = number of voxel reads the ray performed; used only to
- * state the DDA's algorithmic bytes (SURVEY.md section 8d).
+ * state the DDA's algorithmic bytes.
  * ------------------------------------------------------------------------------------------ */
 static inline float axis_t_init(int cell, float o, float d) {
     /* ray_voxel_intersection.cu:95-106 */

@@ -342,7 +342,7 @@ def style_mlp(z, P, prefix='style_net', num_layers=5):
 
 def make_params(seed=0, stress=False, style_dim=128, interm=256, hidden=256, feat=128, nlabels=12, out_c=64,
                 table_entries=16 * (1 << 19), level_dim=8, table_scale=0.1):
-    """Synthetic weights with the reference's state-dict names/shapes (SURVEY.md 8b/8d).
+    """Synthetic weights with the reference's state-dict names/shapes.
 
     stress=False: module default init followed by custom_init (kaiming_normal(a=0.2)*0.5, zero bias;
                   scenedreamer.py:66-78).  Every layer halves the activation RMS, so outputs are ~1e-3.
@@ -392,7 +392,7 @@ def make_params(seed=0, stress=False, style_dim=128, interm=256, hidden=256, fea
         P[s + 'fc%d.bias' % k] = torch.randn(hidden, generator=g) * bg
     P[s + 'fc_out_c.weight'] = kaiming(out_c, hidden, wg * (1.5 if stress else 1.0))
     P[s + 'fc_out_c.bias'] = torch.randn(out_c, generator=g) * bg
-    # hash table (SURVEY 8d: U(-0.1, 0.1) so the encode numerics are exercised)
+    # hash table (U(-0.1, 0.1) so the encode numerics are exercised)
     P['hash_encoder.embeddings'] = (torch.rand(table_entries, level_dim, generator=g) * 2 - 1) * table_scale
     return P
 

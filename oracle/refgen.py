@@ -63,7 +63,7 @@ def setup(backend):
     elif backend == 'ref':
         sys.modules['voxlib'] = _load_ext('ref_voxlib')
         sys.modules['_gridencoder'] = _load_ext('ref_gridencoder')
-        for name in ('upfirdn2d_cuda', 'bias_act_cuda'):       # import-time only (SURVEY 8b); dropin/ ships the product's stand-ins
+        for name in ('upfirdn2d_cuda', 'bias_act_cuda'):       # import-time only; dropin/ ships the product's stand-ins
             sys.modules.setdefault(name, types.ModuleType(name))
     else:
         raise ValueError(backend)

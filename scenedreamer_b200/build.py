@@ -1,10 +1,9 @@
-"""Builds scenedreamer_b200/libsdb200.so (the C-ABI library, include/sdb200.h) with nvcc for sm_100a.
+"""Builds scenedreamer_b200/libsdb200.so (the C-ABI library, include/sdb200.h) with nvcc for sm_90a (H100).
 
     python -m scenedreamer_b200.build [--force] [-v]
 
 Plain nvcc, no torch headers: the library takes raw device pointers + a cudaStream_t, so it
-compiles in seconds and cross-compiles on a box without a GPU.  The .so is built IN-TREE (it is
-git-ignored but travels to the GPU box with the repo snapshot).
+compiles in seconds and cross-compiles on a machine without a GPU.  The .so is built IN-TREE (git-ignored).
 """
 import concurrent.futures
 import hashlib
@@ -17,7 +16,7 @@ CSRC = os.path.join(HERE, 'csrc')
 OBJ = os.path.join(HERE, 'csrc', '_obj')
 LIB = os.path.join(HERE, 'libsdb200.so')
 SOURCES = ['api.cu', 'dda.cu', 'gridenc.cu', 'posenc.cu', 'tc_selftest.cu', 'render_fused.cu', 'render_train.cu', 'wgrad.cu', 'sptrilinear.cu', 'rendercnn.cu', 'optim.cu', 'posestats.cu', 'worldgen.cu', 'modulate.cu']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '-Xcompiler', '-ffp-contract=off', '--expt-relaxed-constexpr'] + \
              os.environ.get('SDB_NVCC_EXTRA', '').split()      # e.g. -DSDB_TIMELINE (diagnostics build)
 
@@ -64,7 +63,7 @@ def build(force=False, verbose=False):
         objs = list(ex.map(cc, srcs))
     # no library dependency besides the CUDA runtime: every kernel on the path, the weight-gradient GEMMs included, is ours
     tmp = LIB + '.tmp.%d' % os.getpid()                       # link aside, then rename: nobody dlopens a half-written file
-    cmd = [nvcc, '-shared', '-o', tmp] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a', '-lcudart']
+    cmd = [nvcc, '-shared', '-o', tmp] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a', '-lcudart']
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError('link failed:\n%s\n%s' % (r.stdout, r.stderr))

@@ -13,8 +13,8 @@ extern "C" int64_t sdb_launch_count(void) { return (int64_t)g_launches.load(std:
 extern "C" int sdb_version(void) { return 100; }  // 0.1.0
 
 extern "C" const char *sdb_build_info(void) {
-    return "libsdb200 0.1.0 sm_100a nvcc " SDB_STR(__CUDACC_VER_MAJOR__) "." SDB_STR(__CUDACC_VER_MINOR__)
-           " (tcgen05/TMEM fused render path, no CPU fallback)";
+    return "libsdb200 0.1.0 sm_90a nvcc " SDB_STR(__CUDACC_VER_MAJOR__) "." SDB_STR(__CUDACC_VER_MINOR__)
+           " (wgmma fused render path, no CPU fallback)";
 }
 
 extern "C" const char *sdb_error_string(int code) {

@@ -1,4 +1,4 @@
-// Shared helpers for libsdb200 (sm_100a only).
+// Shared helpers for libsdb200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -23,9 +23,9 @@ extern "C" void sdb_count_launch_(void);
     } while (0)
 
 static inline int sdb_num_sms() {
-    int dev = 0, n = 148;
+    int dev = 0, n = 132;
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    return n > 0 ? n : 148;
+    return n > 0 ? n : 132;
 }
 
 template <typename T>

@@ -1,11 +1,11 @@
-// a6/a7: stand-alone multi-resolution hash / tiled grid encoder, float32 and (autocast) float16 tables, sm_100a.
+// a6/a7: stand-alone multi-resolution hash / tiled grid encoder, float32 and (autocast) float16 tables, sm_90a.
 //
 // Behavioural contract = _gridencoder.grid_encode_forward / grid_encode_backward of the reference
 // (gridencoder/src/gridencoder.cu:423-478 wrappers; :75-224 kernel_grid, :227-314
 // kernel_grid_backward, :317-343 kernel_input_backward; index math :35-72).  This is the drop-in
 // boundary op; the render hot path itself uses the fused kernel in render_fused.cu.
 //
-// B200 mapping (HBM/L2-gather bound, no tensor cores): one thread per (sample, level); the C
+// GPU mapping (HBM/L2-gather bound, no tensor cores): one thread per (sample, level); the C
 // features of a corner are fetched with ONE vector load (2x LDG.128 for C=8) instead of C scalar
 // loads; the backward scatters with vector reductions (red.global.add.v4.f32, sm_90+) -- 2 per
 // corner for C=8 instead of 8 scalar atomics; blocks are level-major (blockIdx.y = level) so a
@@ -347,9 +347,9 @@ template <uint32_t D, uint32_t C, typename T>
 int launch_fwd(const float *in, const T *emb, const int *off, T *out, uint32_t B, uint32_t L, float S,
                uint32_t H, bool calc, T *dy_dx, uint32_t gt, bool ac, cudaStream_t st) {
     dim3 grid(sdb_div_up(B, 256u), L);
-    // the float32 kernel with dy_dx holds D*C + C accumulators and 2^D gathers in flight: 174 registers at one CTA per SM,
-    // 128 (56 B spilled) at two.  Two is faster at D=5, C=8 (3.98 vs 4.88 ms on 599k samples, profiles/r02_gridenc_minb.log);
-    // SDB_GRIDENC_MINB=1 selects the other build.
+    // the float32 kernel with dy_dx holds D*C + C accumulators and 2^D gathers in flight: two CTAs per SM cap it at 128
+    // registers (a few spills).  Two was the faster choice at D=5, C=8 on the previous GPU generation; carried over, not
+    // re-measured on H100.  SDB_GRIDENC_MINB=1 selects the other build.
     static const int minb = [] { const char *e = getenv("SDB_GRIDENC_MINB"); return e ? atoi(e) : 2; }();
     if (minb == 2 && D * C >= 32)
         grid_forward_kernel<T, D, C, 2><<<grid, 256, 0, st>>>(in, emb, off, out, B, L, S, H, calc, dy_dx, gt, ac);

@@ -1,4 +1,4 @@
-// f2 (SURVEY.md 8(f)-2): the Adam step of the hash table in ONE pass.
+// f2: the Adam step of the hash table in ONE pass.
 // Behavioural contract: torch.optim.Adam as the reference builds it for `hash_encoder.embeddings`
 // (imaginaire/utils/trainer.py:297-323 with configs/scenedreamer_train.yaml:36-61: lr 1e-4, eps 1e-7, betas (0, 0.999), no
 // weight decay, no amsgrad), i.e. per element, with t the step count after the increment:

@@ -1,4 +1,4 @@
-// a9: positional encoding along one dimension, forward + backward, sm_100a.
+// a9: positional encoding along one dimension, forward + backward, sm_90a.
 //
 // Behavioural contract = voxlib.positional_encoding / positional_encoding_backward of the reference
 // (voxlib/positional_encoding_kernel.cu:40-75 forward, :77-118 backward, :125-285 wrappers):

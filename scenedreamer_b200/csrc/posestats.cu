@@ -1,4 +1,4 @@
-// f4 (SURVEY.md 8(f)-4): the two rejection statistics of the training camera sampler, on the device, in one pass.
+// f4: the two rejection statistics of the training camera sampler, on the device, in one pass.
 // Behavioural contract: Generator._get_batch (imaginaire/generators/scenedreamer.py:127-142): after the raycast of a candidate
 // pose,   avg_depth = mean over the non-NaN first-hit entry depths  depth2[0, :, :, 0]            (rejected if < camera_rej_avg_depth)
 //         entropy   = -sum_k p_k log(p_k + 1e-10),  p_k = bincount(voxel_id[:, :, 0], minlength 680) / (H W)   (rejected if < camera_min_entropy)

@@ -1,5 +1,5 @@
-// Fused per-pixel render for sm_100a: depth sampling -> label lookup -> hash-grid features ->
-// style-modulated sigma/colour MLP on tcgen05 tensor cores -> front-to-back compositing + sky blend,
+// Fused per-pixel render for sm_90a: depth sampling -> label lookup -> hash-grid features ->
+// style-modulated sigma/colour MLP on wgmma tensor cores -> front-to-back compositing + sky blend,
 // plus the per-ray sky MLP on the same tensor-core engine.
 //
 // Behavioural contract = Generator._forward_perpix of the reference and the tile loop around it
@@ -12,24 +12,25 @@
 //   volum_rendering_relu + blending      mc_utils.py:154-161, scenedreamer.py:373-413 (a10, a11)
 //
 // Design (DESIGN.md has the long version)
-//   * persistent CTAs (one per SM); a work item is a 16x8-pixel ray tile = 128 rays = the M of one
-//     tcgen05 MMA; row r of every GEMM is ray r, the tile is walked sample by sample (s = 0..S-1),
+//   * persistent CTAs (one per SM); a work item is a 16x8-pixel ray tile = 128 rays = the M of every
+//     GEMM; row r of every GEMM is ray r, the tile is walked sample by sample (s = 0..S-1),
 //     so compositing is a per-thread running sum (no cross-thread reduction, any S);
-//   * warp roles: 8 epilogue warps (TMEM -> LeakyReLU -> 16-bit operand in smem; sigma tap;
+//   * warp roles: 8 epilogue warps (accumulator row -> LeakyReLU -> 16-bit operand in smem; sigma tap;
 //     compositing; warps 0-3 own columns 0..127, warps 4-7 columns 128..255 of the same 128 rows),
-//     1 weight-loader warp (1-D bulk TMA into a ring), 1 MMA-issuer warp, 8 gather warps (hash-grid
-//     fetch for the NEXT sample step while the MLP of the current one runs; results wait in
-//     registers until the operand buffer is free);
-//   * MMA / epilogue overlap: accumulators ping-pong between two 256-column TMEM buffers; layer l+1
-//     starts on a 64-column K chunk as soon as the epilogue of layer l has written it (per-chunk
-//     mbarriers), so the tensor pipe only idles while the first chunk of each layer is produced;
+//     one MMA warpgroup (wgmma in 64x32 blocks; its thread 0 also streams the weights into a 4-slot ring
+//     with 1-D bulk TMA copies), 8 gather warps (hash-grid fetch for the NEXT sample step while the MLP
+//     of the current one runs; results wait in registers until the operand buffer is free);
+//   * accumulators: a layer's fp32 [128 x 256] result (128 KB) fits neither next to the operand buffers in
+//     shared memory nor in the registers the three roles share, so the MMA warpgroup writes it to a
+//     per-CTA buffer pair in global memory (L2-resident, ping-pong by layer parity) and the epilogue reads
+//     its rows from there; a layer starts when the epilogue has written all of its input;
 //   * bias, style beta and the label embedding ride in the GEMM: the operand has 16 extra K columns
 //     (one-hot label + constant 1), the weight image carries bias / embedding rows there -- exactly
 //     the reference's fc_m_a(onehot) product -- so the epilogue is LeakyReLU + 16-bit split only;
-//   * activations stay on chip: TMEM accumulators and ONE in-place 128x272 operand buffer in shared
-//     memory; the only per-sample HBM/L2 traffic is the table gather;
+//   * the 16-bit activations stay on chip: ONE in-place 128x272 operand buffer in shared memory; the
+//     per-sample L2 traffic is the table gather plus the accumulator round trip above;
 //   * precision: 0 = one fp16 pass; 1 / 2 = bf16 / fp16 "x3" split (x_hi*W_hi + x_lo*W_hi + x_hi*W_lo:
-//     ~2^-16 resp. ~2^-21 relative, i.e. fp32-grade for the 1e-3 parity bar); accumulation is fp32 in TMEM;
+//     ~2^-16 resp. ~2^-21 relative, i.e. fp32-grade for the 1e-3 parity bar); accumulation is fp32;
 //   * sky-only tiles never reach the render kernel: a pre-pass writes their outputs and compacts the
 //     list of live tiles (their compositing weights are exactly zero, scenedreamer.py:376).
 //   * early termination + dynamic tile scheduling (inference): a tile stops marching once every live ray is opaque
@@ -38,6 +39,10 @@
 //     data-gradient chains (MODE kBwd / kSkyBwd: transposed weights, LeakyReLU' from recorded sign words);
 //     render_train.cu holds the rest of the backward (compositing, table scatter, weight-gradient GEMMs).
 #include <stdlib.h>
+
+#include <map>
+#include <mutex>
+#include <utility>
 
 #include "rf_common.cuh"
 
@@ -131,7 +136,7 @@ __device__ __forceinline__ void encode_level(const float *__restrict__ tbl, uint
 
 // encode_level<false> with at most 2 * GU gathers of a lane in flight (the corner loop is unrolled GU times only): the ray-slot
 // kernel's gather shares the LSU with the epilogue's operand stores, and a fully unrolled level queues 16 scattered LDG.128 per
-// lane -- up to 4,096 L1 wavefronts ahead of every epilogue store (profiles/r02_render_timeline.txt).  Same arithmetic per feature.
+// lane -- up to 4,096 L1 wavefronts ahead of every epilogue store.  Same arithmetic per feature.
 template <int GU>
 __device__ __forceinline__ void encode_level_thin(const float *__restrict__ tbl, uint32_t mask, float scale, const float (&x)[5],
                                                   float (&res)[8]) {
@@ -216,9 +221,6 @@ mlp_kernel(const Params p)
     constexpr Smem SM = smem_map(X3);
     constexpr int PARTS = X3 ? 2 : 1;
     constexpr int NH = Net<MODE>::NH, NL = Net<MODE>::NL;
-    constexpr int KS = X3 ? 1 : 2;                           // k16 slabs per ring stage
-    constexpr int kStageBytes = KS * kHidden * 32 * PARTS;   // 16 KB either way
-    constexpr int kStages = kRingBytes / kStageBytes;        // 4
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t *sHhi = smem + SM.h_hi;
     uint8_t *sHlo = smem + SM.h_lo;
@@ -229,7 +231,6 @@ mlp_kernel(const Params p)
     float *sSig = reinterpret_cast<float *>(smem + SM.sig);
     float *sState = reinterpret_cast<float *>(smem + SM.state);
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem + SM.bars);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(smem + SM.tmem_slot);
     // Early termination (north star: "early termination"; inference render only).  stop_step[buf] = number of sample
     // steps the tile in state buffer `buf` executes (S until decided).  The epilogue decides during the compositing of
     // step s ("every live ray has transmittance < early_T") and sets s + 2: by the time ANY role starts step s + 2 it
@@ -257,8 +258,7 @@ mlp_kernel(const Params p)
 
     // ---- one-time setup ----
     if (tid == 0) {
-        static_assert(kStages <= 4, "barrier table holds 4 ring stages");
-        for (int i = 0; i < 4; i++) { tc05::mbar_init(&bars[B_WFULL + i], 1); tc05::mbar_init(&bars[B_WEMPTY + i], 1); }
+        for (int i = 0; i < 4; i++) tc05::mbar_init(&bars[B_WFULL + i], 1);
         tc05::mbar_init(&bars[B_FEAT], kGatherThreads);
         tc05::mbar_init(&bars[B_HFREE], 1);
         for (int i = 0; i < 16; i++) tc05::mbar_init(&bars[B_CHUNK + i], kEpiThreads / 2);
@@ -270,7 +270,6 @@ mlp_kernel(const Params p)
         tc05::mbar_init(&bars[B_COMP], kEpiThreads);
         tc05::fence_mbar_init();
     }
-    if (warp == kLoaderWarp) tc05::tmem_alloc(tmem_slot, kTmemCols);
     if (tid < 2) { sStop[tid] = RAYQ ? 0x7fffffff : kMaxS + 1; sVote[tid] = 0; }
     if constexpr (RAYQ) {
         for (int i = tid; i < kRows; i += kThreads) { sCur[i] = make_int2(-1, 0); sDone[i] = 0; sDone[kRows + i] = 0; }
@@ -306,16 +305,13 @@ mlp_kernel(const Params p)
         if constexpr (X3) *reinterpret_cast<uint4 *>(sHlo + tc05::chunk_off(kRows, r, kc)) = make_uint4(0, 0, 0, 0);
     }
     tc05::fence_proxy_async_smem();
-    tc05::fence_before_thread_sync();
     __syncthreads();
-    tc05::fence_after_thread_sync();
-    const uint32_t tmem = *tmem_slot;
     const uint32_t mask = SKY ? 0u : ((1u << p.log2_T) - 1u);
 
     if (warp < 8) {
         // =========================== EPILOGUE / COMPOSITING WARPS ===========================
         const int row = tid & (kRows - 1), half = tid >> 7;          // column half: 128*half .. +127
-        const uint32_t tm_row = tmem + ((uint32_t)((warp & 3) * 32) << 16);
+        const float *acc_row = p.acc + (size_t)blockIdx.x * 2 * kRows * kHidden + (size_t)row * kHidden;   // accumulator row
         uint32_t n = 0;                 // global step counter
         int loaded_img = -1;
         for (int it = 0;; it++) {
@@ -374,7 +370,7 @@ mlp_kernel(const Params p)
 #pragma unroll 1
                 for (int l = 0; l < NH; l++) {
                     const uint32_t g = n * NL + l;                   // global layer counter -> accumulator buffer
-                    const uint32_t acc = tm_row + (g & 1u) * 256u + half * 128u;
+                    const float *acc = acc_row + (g & 1u) * kRows * kHidden + half * 128;
                     // kBwd: LeakyReLU sign words of the forward activation A_{6-l} this layer's data gradient passes
                     // through (prefetched before the accumulator wait)
                     uint4 mw = make_uint4(0u, 0u, 0u, 0u);
@@ -382,7 +378,6 @@ mlp_kernel(const Params p)
                         mw = __ldg(reinterpret_cast<const uint4 *>(p.tr.mask + ((step_id * kNumAct + (NACT - 1 - l)) * kRows + row) * 8 + half * 4));
                     if ((tid & 127) == 0) SDB_MARK(half, 1, n, l);
                     tc05::mbar_wait(&bars[B_ACC], (n * NH + l) & 1);
-                    tc05::fence_after_thread_sync();
                     if ((tid & 127) == 0) SDB_MARK(half, 2, n, l);
                     if ((tid & 127) == 0) SDB_STAMP(n, l, 2 + 2 * half);
 #pragma unroll 1
@@ -397,8 +392,7 @@ mlp_kernel(const Params p)
 #pragma unroll
                         for (int hh = 0; hh < 2; hh++) {
                             float v[16];
-                            tc05::tmem_ld16(acc + c0 + 16 * hh, v);
-                            tc05::tmem_ld_wait();
+                            acc_ld<16>(acc + c0 + 16 * hh, v);
                             if constexpr (BWD) {
                                 if (MODE == kBwd && l == 2) {   // dA4 += dsigma * fc_sigma.weight (sigma taps A4, layers.py:115)
                                     const float *ws = sF + kFWsig + half * 128 + c0 + 16 * hh;
@@ -454,7 +448,6 @@ mlp_kernel(const Params p)
                         }
                         if constexpr (TRAIN) p.tr.mask[((step_id * kNumAct + l) * kRows + row) * 8 + half * 4 + (c0 >> 5)] = mword;
                     }
-                    tc05::fence_before_thread_sync();
                     tc05::mbar_arrive(&bars[B_EPIDONE + (g & 1u)]);        // accumulator buffer (g & 1) is free again
                     if ((tid & 127) == 0) SDB_STAMP(n, l, 3 + 2 * half);
                     if (MODE == kRender && l == 3) sSig[half * kRows + row] = sig_part;
@@ -472,15 +465,13 @@ mlp_kernel(const Params p)
                 tc05::mbar_wait(&bars[B_OUTRDY], n & 1);
                 if ((tid & 127) == 0) SDB_MARK(half, 4, n, NH);
                 if ((tid & 127) == 0) SDB_STAMP(n, NH, 2 + 2 * half);
-                tc05::fence_after_thread_sync();
                 if constexpr (SKYBWD) {
                     // last layer of the sky chain: dA1 [128 x 256] -> dZ1 = dA1 * LeakyReLU'(z1) -> bf16 record only
                     const uint4 mw = __ldg(reinterpret_cast<const uint4 *>(p.tr.mask + ((step_id * kNumAct + 0) * kRows + row) * 8 + half * 4));
 #pragma unroll 1
                     for (int c0 = 0; c0 < 128; c0 += 32) {
                         float v[32];
-                        tc05::tmem_ld32(tm_row + (go & 1u) * 256u + half * 128u + c0, v);
-                        tc05::tmem_ld_wait();
+                        acc_ld<32>(acc_row + (go & 1u) * kRows * kHidden + half * 128 + c0, v);
                         const uint32_t word = c0 == 0 ? mw.x : (c0 == 32 ? mw.y : (c0 == 64 ? mw.z : mw.w));
 #pragma unroll
                         for (int j = 0; j < 32; j++) v[j] = ((word >> j) & 1u) ? v[j] : 0.2f * v[j];
@@ -491,22 +482,17 @@ mlp_kernel(const Params p)
                                 make_uint4(tc05::pack2<true>(v[8 * q], v[8 * q + 1]), tc05::pack2<true>(v[8 * q + 2], v[8 * q + 3]),
                                            tc05::pack2<true>(v[8 * q + 4], v[8 * q + 5]), tc05::pack2<true>(v[8 * q + 6], v[8 * q + 7]));
                     }
-                    tc05::fence_before_thread_sync();
                     tc05::mbar_arrive(&bars[B_EPIDONE + (go & 1u)]);
-                if ((tid & 127) == 0) SDB_STAMP(n, NH, 3 + 2 * half);
                     if ((tid & 127) == 0) SDB_STAMP(n, NH, 3 + 2 * half);
                     continue;
                 }
                 float c[32];
-                tc05::tmem_ld32(tm_row + (go & 1u) * 256u + half * (BWD ? 64u : 32u), c);
+                acc_ld<32>(acc_row + (go & 1u) * kRows * kHidden + half * (BWD ? 64 : 32), c);
                 if constexpr (BWD) {
                     // d(hash-grid features) [128 rays x 128]: this half owns 64 columns -> fp32 record for the table backward
                     float c2[32];
-                    tc05::tmem_ld32(tm_row + (go & 1u) * 256u + half * 64u + 32u, c2);
-                    tc05::tmem_ld_wait();
-                    tc05::fence_before_thread_sync();
+                    acc_ld<32>(acc_row + (go & 1u) * kRows * kHidden + half * 64 + 32, c2);
                     tc05::mbar_arrive(&bars[B_EPIDONE + (go & 1u)]);
-                if ((tid & 127) == 0) SDB_STAMP(n, NH, 3 + 2 * half);
                     if ((tid & 127) == 0) SDB_STAMP(n, NH, 3 + 2 * half);
                     float *dst = p.tr.dx0 + slot * kFeat + half * 64;
 #pragma unroll
@@ -515,8 +501,6 @@ mlp_kernel(const Params p)
                     for (int q = 0; q < 4; q++) st_global_v8f(dst + 32 + 8 * q, &c2[8 * q]);
                     continue;
                 }
-                tc05::tmem_ld_wait();
-                tc05::fence_before_thread_sync();
                 tc05::mbar_arrive(&bars[B_EPIDONE + (go & 1u)]);
                 if ((tid & 127) == 0) SDB_STAMP(n, NH, 3 + 2 * half);
                 if constexpr (SKY) {
@@ -713,145 +697,126 @@ mlp_kernel(const Params p)
         }
     } else if (warp < kGatherWarp0) {
       asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegsCtl));
-      constexpr int NSP = stages_per_step_padded<KS, MODE>();      // ring stages per sample step (multiple of 4)
-      constexpr int NS = stages_per_step<KS, MODE>();
-      constexpr uint32_t kStepFlip = (NSP / 4) & 1;                 // does the stage parity pattern flip every step?
-      static_assert(kStages == 4, "static schedule assumes a 4-deep ring");
-      if (warp == kLoaderWarp) {
-        // =========================== WEIGHT LOADER (1-D bulk TMA) ===========================
-        if (lane == 0) {
-            uint32_t n = 0;
-            for (int it = 0;; it++) {
-                const int work = fetch_work(it);
-                if (work < 0) break;
-                const int tile = RAYQ ? 0 : (ONE_STEP ? work : p.tile_list[work / wmult]);
-                const TileCoord tc = tile_coord(p, tile);
-                const uint8_t *pack = p.pack + (long long)tc.img * p.pack_stride;
-                for (int s = 0; s < SL; s++, n++) {
-                    if (ESTOP && s >= 2 && s >= sStop[it & 1]) break;
-                    const uint32_t flip = kStepFlip & n;
+      // =========================== MMA WARPGROUP ===========================
+      // Layer l of a sample step: D[128 x N] = H[128 x K] * W_l^T, computed in 64-row x 32-column blocks (the sum over K in
+      // registers), each written once to this CTA's fp32 accumulator buffer (g & 1) in global memory, where the epilogue reads
+      // its rows.  Weights go through a 4-slot ring of 16 KB stages = up to 8 k16 slabs of one 32-column block; thread 0
+      // issues the bulk copies up to 3 stages ahead of the MMAs.  Named barrier 3 is this warpgroup's (1: epilogue, 2: gather).
+      const int t = tid - kMmaWarp0 * 32;
+      constexpr uint32_t kSlot = 16384, kSlabB = 1024 * PARTS;       // ring slot; one k16 slab of a 32-column block
+      uint32_t n = 0, q0 = 0;                                        // q0: ring stages of all earlier steps
+      auto layer_stages = [&](int l) { return 2 * (layerN<MODE>(l) / 32) * ((layerK<MODE>(l) / 16 + 7) / 8); };
+      for (int it = 0;; it++) {
+          const int work = fetch_work(it);
+          if (work < 0) break;
+          const int tile = RAYQ ? 0 : (ONE_STEP ? work : p.tile_list[work / wmult]);
+          const uint8_t *pack = p.pack + (long long)tile_coord(p, tile).img * p.pack_stride;
+          int n_st = 0;
+          for (int l = 0; l < NL; l++) n_st += layer_stages(l);
+          // stage k of a step -> (layer, 32-column block, first slab, slabs); stages go (layer, row block, column block, slabs)
+          auto issue = [&](int k) {
+              int l = 0;
+              while (k >= layer_stages(l)) { k -= layer_stages(l); l++; }
+              const int N = layerN<MODE>(l), nK = layerK<MODE>(l) / 16, nsg = (nK + 7) / 8;
+              const int blk = k / nsg, sg = k % nsg, cc = blk % (N / 32);
+              const int kk0 = sg * 8;
+              return make_int4(l, cc, kk0, min(8, nK - kk0));
+          };
+          for (int s = 0; s < SL; s++, n++) {
+              if (ESTOP && s >= 2 && s >= sStop[it & 1]) break;
+              int k = 0, k_issued = 0;
+              auto produce = [&](int upto) {           // thread 0: stages k_issued .. upto - 1 of this step
+                  for (; k_issued < upto && k_issued < n_st; k_issued++) {
+                      const int4 d = issue(k_issued);
+                      const int N = layerN<MODE>(d.x);
+                      const uint32_t q = q0 + (uint32_t)k_issued, slot = q & 3u;
+                      const uint8_t *w = pack + layerOff<MODE>(d.x, PARTS);
+                      const uint32_t slabB = (uint32_t)N * 32u * PARTS;
+                      tc05::mbar_arrive_expect_tx(&bars[B_WFULL + slot], (uint32_t)d.w * kSlabB);
+                      for (int i = 0; i < d.w; i++)
 #pragma unroll
-                    for (int l = 0; l < NL; l++) {
-                        const uint32_t slabB = (uint32_t)layerN<MODE>(l) * 32 * PARTS;      // one k16 slab (hi [+ lo])
-                        const uint8_t *src = pack + layerOff<MODE>(l, PARTS);
+                          for (int part = 0; part < PARTS; part++)
 #pragma unroll
-                        for (int j = 0; j < num_stages<KS, MODE>(l); j++) {
-                            const int i = stage_index<KS, MODE>(l, j);
-                            const uint32_t stg = i & 3, par = ((i >> 2) & 1) ^ flip;
-                            const uint32_t bytes = slabB * stage_cnt<KS, MODE>(l, j);
-                            tc05::mbar_wait_backoff(&bars[B_WEMPTY + stg], par ^ 1, 32);
-                            tc05::mbar_arrive_expect_tx(&bars[B_WFULL + stg], bytes);
-                            tc05::bulk_g2s(sRing + stg * kStageBytes, src + (size_t)stage_kk<KS, MODE>(l, j) * slabB, bytes,
-                                           &bars[B_WFULL + stg]);
-                        }
-                    }
+                              for (int kc = 0; kc < 2; kc++)
+                                  tc05::bulk_g2s(sRing + slot * kSlot + i * kSlabB + part * 1024 + kc * 512,
+                                                 w + (size_t)(d.z + i) * slabB + part * N * 32 + kc * N * 16 + d.y * 512, 512,
+                                                 &bars[B_WFULL + slot]);
+                  }
+              };
+              if (t == 0) produce(3);
+#pragma unroll 1
+              for (int l = 0; l < NL; l++) {
+                  const uint32_t g = n * NL + l, buf = g & 1u;
+                  if (t == 0) SDB_MARK(2, 1, n, l);
+                  // accumulator buffer `buf` was last read by the epilogue of global layer g - 2
+                  if (g >= 2) tc05::mbar_wait(&bars[B_EPIDONE + buf], ((g >> 1) - 1) & 1);
+                  if (l == 0) {
+                      tc05::mbar_wait(&bars[B_FEAT], n & 1);
+                  } else {
+                      const uint32_t cpar = (n * NH + l - 1) & 1;      // operand of this layer from the previous epilogue
+                      for (int c = 0; c < 16; c++) tc05::mbar_wait(&bars[B_CHUNK + c], cpar);
+                  }
+                  if (t == 0) SDB_MARK(2, 2, n, l);
+                  if (t == 0) SDB_STAMP(n, l, 0);
+                  const int N = layerN<MODE>(l), nK = layerK<MODE>(l) / 16, nsg = (nK + 7) / 8;
+                  float *dst = p.acc + ((size_t)blockIdx.x * 2 + buf) * kRows * kHidden;
+#pragma unroll 1
+                  for (int rb = 0; rb < 2; rb++) {
+#pragma unroll 1
+                      for (int cc = 0; cc < N / 32; cc++) {
+                          float d[16], sum[16];
+#pragma unroll 1
+                          for (int sg = 0; sg < nsg; sg++, k++) {
+                              if (t == 0) produce(k + 4);
+                              const uint32_t q = q0 + (uint32_t)k, slot = q & 3u;
+                              tc05::mbar_wait(&bars[B_WFULL + slot], (q >> 2) & 1u);
+                              const uint32_t sb = tc05::smem_u32(sRing + slot * kSlot);
+                              const int kk0 = sg * 8, ns = min(8, nK - kk0);
+                              tc05::wgmma_fence();
+#pragma unroll 1
+                              for (int i = 0; i < ns; i++) {
+                                  const uint32_t aoff = (uint32_t)(kk0 + i) * 2 * kLboA + rb * 1024;
+                                  const uint64_t ah = tc05::make_smem_desc(tc05::smem_u32(sHhi) + aoff, kLboA, kSbo);
+                                  const uint64_t bh = tc05::make_smem_desc(sb + i * kSlabB, 512, kSbo);
+                                  tc05::wgmma_m64n32k16<BF16, 0, 0>(d, ah, bh, i > 0 ? 1u : 0u);
+                                  if constexpr (X3) {
+                                      const uint64_t al = tc05::make_smem_desc(tc05::smem_u32(sHlo) + aoff, kLboA, kSbo);
+                                      tc05::wgmma_m64n32k16<BF16, 0, 0>(d, al, bh, 1u);
+                                      tc05::wgmma_m64n32k16<BF16, 0, 0>(d, ah, bh + (1024 >> 4), 1u);
+                                  }
+                              }
+                              tc05::wgmma_commit();
+                              tc05::wgmma_wait<0>();
+                              tc05::wgmma_fence_acc(d);
+                              tc05::named_sync(3, 128);           // every warp is done with the slot: it may be refilled
+                              // Every stage (<= 8 k16 slabs) starts a fresh tensor-core sum, added to the running sum in fp32
+                              // with round-to-nearest: the tensor core's own accumulation does not round to nearest, and over a
+                              // whole x3 layer (up to 51 chained MMAs) that moved the full-frame depth outside its parity bound.
 #pragma unroll
-                    for (int i = NS; i < NSP; i++) {       // padding stages: a 16-byte dummy transaction keeps the phases regular
-                        const uint32_t stg = i & 3, par = ((i >> 2) & 1) ^ flip;
-                        tc05::mbar_wait_backoff(&bars[B_WEMPTY + stg], par ^ 1, 32);
-                        tc05::mbar_arrive_expect_tx(&bars[B_WFULL + stg], 16);
-                        tc05::bulk_g2s(sRing + stg * kStageBytes, pack, 16, &bars[B_WFULL + stg]);
-                    }
-                }
-            }
-        }
-      } else if (warp == kMmaWarp) {
-        // =========================== MMA ISSUER ===========================
-        // The warp stays converged (uniform control flow, every lane polls the barriers), one elected lane
-        // issues tcgen05.mma / commit.  Ring slot, barrier addresses, parities and descriptor offsets of every
-        // stage are immediates (static schedule above) and two ring stages are issued per iteration, so the
-        // fixed cost of an iteration (~40 instructions of a single warp) is amortised over up to 6 MMAs.
-        // (Earlier versions spent ~600 cycles per k16 step in this loop and capped the tensor pipe at ~50 %,
-        // profiles/r01_v2b_*.)
-        uint32_t n = 0;
-        const uint64_t dA0h = tc05::make_smem_desc(tc05::smem_u32(sHhi), kLboA, kSbo);
-        const uint64_t dA0l = tc05::make_smem_desc(tc05::smem_u32(sHlo), kLboA, kSbo);
-        const uint64_t dB0_256 = tc05::make_smem_desc(tc05::smem_u32(sRing), 256 * 16, kSbo);
-        const uint64_t dB0_64 = tc05::make_smem_desc(tc05::smem_u32(sRing), kOutC * 16, kSbo);
-        const uint64_t dB0_128 = tc05::make_smem_desc(tc05::smem_u32(sRing), kFeat * 16, kSbo);
-        for (int it = 0;; it++) {
-            if (fetch_work(it) < 0) break;                              // warp-uniform
-            for (int s = 0; s < SL; s++, n++) {
-                if (ESTOP && s >= 2 && s >= sStop[it & 1]) break;       // warp-uniform (same shared word for every lane)
-                const uint32_t flip = kStepFlip & n;
-                const uint32_t nodd = n & 1u;
+                              for (int i = 0; i < 16; i++) sum[i] = sg == 0 ? d[i] : __fadd_rn(sum[i], d[i]);
+                          }
+#ifndef SDB_AB_NO_ACC
 #pragma unroll
-                for (int l = 0; l < NL; l++) {
-                    const uint32_t g = n * NL + l;
-                    const uint32_t buf = ((nodd * (NL & 1)) ^ (l & 1)) & 1u;      // == g & 1
-                    // accumulator buffer `buf` was last read by the epilogue of global layer g-2.  One
-                    // barrier PER BUFFER: its next completion needs this layer's own MMAs, so the parity
-                    // wait can never fall two phases behind (a single shared barrier can: the 64-column
-                    // colour layer finishes within a few hundred cycles).
-                    if (lane == 0) SDB_MARK(2, 1, n, l);
-                    if (g >= 2) tc05::mbar_wait(&bars[B_EPIDONE + buf], ((g >> 1) - 1) & 1);
-                    if (l == 0) tc05::mbar_wait(&bars[B_FEAT], nodd);
-                    if (lane == 0) SDB_STAMP(n, l, 0);
-                    const int N = layerN<MODE>(l);                                  // compile-time after unrolling
-                    const uint32_t idesc = tc05::make_idesc(kRows, N, BF16);
-                    const uint32_t slab16 = (uint32_t)(N * 32) >> 4;              // one part of one k16 slab, in 16-byte units
-                    const uint32_t dcol = tmem + buf * 256u;
-                    const uint64_t dB0 = (N == kOutC) ? dB0_64 : (N == kFeat ? dB0_128 : dB0_256);
-                    const uint32_t cpar = (NH & 1) ? (((l - 1) & 1) ^ nodd) : ((l - 1) & 1);   // (n*NH + l-1) & 1
-                    constexpr int kPair = 2;
-#pragma unroll
-                    for (int j0 = 0; j0 < num_stages<KS, MODE>(l); j0 += kPair) {
-#pragma unroll
-                        for (int u = 0; u < kPair; u++) {
-                            const int j = j0 + u;
-                            if (j < num_stages<KS, MODE>(l)) {
-                                const int i = stage_index<KS, MODE>(l, j);
-                                const int chunk = stage_chunk_wait<KS, MODE>(l, j);
-                                if (chunk >= 0) tc05::mbar_wait(&bars[B_CHUNK + chunk], cpar);   // operand chunk from the previous epilogue
-                                tc05::mbar_wait(&bars[B_WFULL + (i & 3)], ((i >> 2) & 1) ^ flip);
-                            }
-                        }
-                        tc05::fence_after_thread_sync();
-                        if (elect_one()) {
-#pragma unroll
-                            for (int u = 0; u < kPair; u++) {
-                                const int j = j0 + u;
-                                if (j < num_stages<KS, MODE>(l)) {
-                                    const int i = stage_index<KS, MODE>(l, j);
-                                    const uint32_t stg = i & 3;
-                                    const uint64_t dBs = dB0 + (uint64_t)(stg * (kStageBytes >> 4));
-#pragma unroll
-                                    for (int t = 0; t < stage_cnt<KS, MODE>(l, j); t++) {
-                                        const int kk = stage_kk<KS, MODE>(l, j) + t;
-                                        const uint64_t dAh = dA0h + (uint64_t)(kk * (2 * kLboA >> 4));
-                                        const uint64_t dBh = dBs + (uint64_t)(t * slab16 * PARTS);
-                                        const bool first = (j == 0 && t == 0);
-                                        tc05::mma_f16_ss(dcol, dAh, dBh, idesc, first ? 0u : 1u);
-                                        if constexpr (X3) {
-                                            const bool ext = (Net<MODE>::EXT && l > 0 && j == 0);   // A_lo of the constant extension columns is 0
-                                            if (!ext) tc05::mma_f16_ss(dcol, dA0l + (uint64_t)(kk * (2 * kLboA >> 4)), dBh, idesc, 1u);
-                                            tc05::mma_f16_ss(dcol, dAh, dBh + slab16, idesc, 1u);
-                                        }
-                                    }
-                                    tc05::mma_commit(&bars[B_WEMPTY + stg]);
-                                    if (j == num_stages<KS, MODE>(l) - 1) {
-                                        SDB_STAMP(n, l, 1);
-                                        if (l == NL - 1) {
-                                            tc05::mma_commit(&bars[B_OUTRDY]);
-                                            tc05::mma_commit(&bars[B_HFREE]);
-                                        } else {
-                                            tc05::mma_commit(&bars[B_ACC]);
-                                        }
-                                    }
-                                }
-                            }
-                        }
-                        __syncwarp();
-                    }
-                }
-#pragma unroll
-                for (int i = NS; i < NSP; i++) {       // padding stages (see loader)
-                    tc05::mbar_wait(&bars[B_WFULL + (i & 3)], ((i >> 2) & 1) ^ flip);
-                    if (elect_one()) tc05::mma_commit(&bars[B_WEMPTY + (i & 3)]);
-                    __syncwarp();
-                }
-            }
-        }
+                          for (int i = 0; i < 16; i += 2)
+                              *reinterpret_cast<float2 *>(dst + (size_t)(rb * 64 + tc05::frag_row(t, i)) * kHidden + cc * 32 +
+                                                          tc05::frag_col(t, i)) = make_float2(sum[i], sum[i + 1]);
+#endif
+                      }
+                  }
+                  __threadfence_block();
+                  tc05::named_sync(3, 128);
+                  if (t == 0) SDB_STAMP(n, l, 1);
+                  if (t == 0) {
+                      if (l == NL - 1) {
+                          tc05::mbar_arrive(&bars[B_OUTRDY]);
+                          tc05::mbar_arrive(&bars[B_HFREE]);
+                      } else {
+                          tc05::mbar_arrive(&bars[B_ACC]);
+                      }
+                  }
+              }
+              q0 += (uint32_t)n_st;
+          }
       }
     } else {
         // =========================== GATHER WARPS (layer-0 operand producers) ===========================
@@ -1232,9 +1197,6 @@ mlp_kernel(const Params p)
             }
         }
     }
-    tc05::fence_before_thread_sync();
-    __syncthreads();
-    if (warp == kLoaderWarp) tc05::tmem_dealloc(tmem, kTmemCols);
 }
 
 // ---- pre-pass: live-tile list + outputs of sky-only tiles -----------------------------------------
@@ -1471,8 +1433,35 @@ int launch_pack(const float *w0, const float *b0, const float *emb, int n_labels
     return SDB_OK;
 }
 
+// Per-CTA fp32 accumulator buffers of the fused kernels ([grid][2][128][256], L2-resident), one per (device, stream): launches
+// on one stream are ordered, so they can share it; launches on different streams get different buffers.  A buffer is
+// allocated (or grown) on the first launch that needs it and kept for the life of the process.  Allocation is refused while
+// the stream is being captured into a CUDA graph: run one launch of the same size outside the capture first.
+static int acc_buffers(int grid, cudaStream_t st, float **out) {
+    static std::mutex mu;
+    static std::map<std::pair<int, cudaStream_t>, std::pair<float *, int>> bufs;
+    int dev = 0;
+    SDB_CUDA(cudaGetDevice(&dev));
+    std::lock_guard<std::mutex> lk(mu);
+    std::pair<float *, int> &b = bufs[std::make_pair(dev, st)];
+    if (b.second < grid) {
+        cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+        SDB_CUDA(cudaStreamIsCapturing(st, &cs));
+        if (cs != cudaStreamCaptureStatusNone) return SDB_EUNSUPPORTED;
+        if (b.first) SDB_CUDA(cudaFree(b.first));
+        b = std::make_pair((float *)nullptr, 0);
+        SDB_CUDA(cudaMalloc(&b.first, (size_t)grid * 2 * kRows * kHidden * sizeof(float)));
+        b.second = grid;
+    }
+    *out = b.first;
+    return SDB_OK;
+}
+
 template <int PREC, bool RAW5D, int MODE, bool TRAIN = false, bool RAYQ = false, int GU = 8>
-int launch_mlp(const Params &p, int grid, cudaStream_t st) {
+int launch_mlp(const Params &p_in, int grid, cudaStream_t st) {
+    Params p = p_in;
+    const int e = acc_buffers(grid, st, &p.acc);
+    if (e != SDB_OK) return e;
     const size_t smem = smem_map(PREC != 0).total;
     cudaFuncAttributes fa;
     SDB_CUDA(cudaFuncGetAttributes(&fa, mlp_kernel<PREC, RAW5D, MODE, TRAIN, RAYQ, GU>));
@@ -1755,8 +1744,8 @@ extern "C" int sdb_render_rays_forward(const sdb_render_params *sp, void *stream
         if (sp->precision == 0) rc = launch_mlp<0, false, kRender, false, true>(p, grid, st);
         else if (sp->precision == 1) rc = launch_mlp<1, false, kRender, false, true>(p, grid, st);
         else {
-            // gathers in flight per lane: 2 corners (4 LDG.128) measured best -- kernel 9.48 ms vs 9.81 fully unrolled, 9.68 / 9.53 at
-            // 4 / 1 corners (profiles/r02_exp_gather_unroll.json); SDB_GATHER_UNROLL=8 selects the fully unrolled level
+            // gathers in flight per lane: 2 corners (4 LDG.128) by default, a choice measured on the previous GPU generation and not
+            // re-measured on H100; SDB_GATHER_UNROLL=8 selects the fully unrolled level
             static const int gu = [] { const char *e = getenv("SDB_GATHER_UNROLL"); return e ? atoi(e) : 2; }();
             if (gu == 8) rc = launch_mlp<2, false, kRender, false, true>(p, grid, st);
             else rc = launch_mlp<2, false, kRender, false, true, 2>(p, grid, st);

@@ -1,4 +1,4 @@
-// Training side of the fused per-pixel path (a7 + the backward of a8/a10/a11), sm_100a.
+// Training side of the fused per-pixel path (a7 + the backward of a8/a10/a11), sm_90a.
 //
 // Behavioural contract = what torch.autograd computes for Generator._forward_perpix in the reference under
 // train.py (imaginaire/generators/scenedreamer.py:313-428): gradients of net_out with respect to
@@ -7,17 +7,17 @@
 //   the sky features (-> sky_net)                  scenedreamer.py:387-413
 // through volum_rendering_relu (mc_utils.py:154-161), clamp and the sky blend (scenedreamer.py:373-413).
 //
-// B200 mapping ("split-fused", DESIGN.md section 3.6): the forward pass (render_fused.cu, TRAIN variant) leaves a
+// GPU mapping ("split-fused", DESIGN.md section 3.6): the forward pass (render_fused.cu, TRAIN variant) leaves a
 // per-sample record in HBM (about 3.9 KB per sample -- 6.7 GB for a 256x256x24 training view, a few per cent of the
 // 180 GB), then
 //   1. composite_backward_kernel  : one warp per ray, lanes over the 64 feature channels / the S samples;
-//   2. mlp_kernel<bf16x3, kBwd>   : the data-gradient chain on the same tcgen05 engine as the forward
+//   2. mlp_kernel<bf16x3, kBwd>   : the data-gradient chain on the same wgmma engine as the forward
 //                                   (transposed weights in the ring, LeakyReLU' from recorded sign words);
 //   3. table3_backward_kernel     : scatter into the PRE-BLENDED 3-D table (8 corners instead of 32, vector
 //                                   red.add), then the transpose of the pre-blend (the same gather kernel:
 //                                   XOR-indexing is an involution) and the scene-code gradient;
 //   4. weight gradients           : dZ^T * A over all samples on the tensor cores (wgrad.cu): the bf16 records are
-//                                   MMA-ready tiles, bulk-copied into shared memory, fp32 accumulators in TMEM.
+//                                   MMA-ready tiles, bulk-copied into shared memory, fp32 accumulators in registers.
 #include <stdio.h>
 #include <stdlib.h>
 
@@ -479,7 +479,8 @@ extern "C" int sdb_render_rays_backward(const sdb_render_params *sp, const void 
     // 3. table gradient: scatter into the pre-blended table, transpose of the pre-blend, scene code
     {
         dim3 grid((unsigned)((cap_items * kRows + 255) / 256), kLevels);
-        // SDB_TABLE_AGG_LEVELS: tuning knob (levels 0..n-1 use the warp-aggregated scatter); default from profiles/
+        // SDB_TABLE_AGG_LEVELS: tuning knob (levels 0..n-1 use the warp-aggregated scatter); the default was chosen on the
+        // previous GPU generation and is carried over, not re-measured on H100
         int agg_levels = 12;
         if (const char *e = getenv("SDB_TABLE_AGG_LEVELS")) agg_levels = atoi(e);
         table3_backward_kernel<<<grid, 256, 0, st>>>(p, dx0, dt3, agg_levels);

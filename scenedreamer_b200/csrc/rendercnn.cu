@@ -1,27 +1,28 @@
-// RenderCNN + tanh on the tcgen05 tensor cores (sm_100a): the step right after the per-pixel path (SURVEY.md 8(f)-1).
+// RenderCNN + tanh on the Hopper tensor cores (sm_90a, wgmma): the step right after the per-pixel path.
 // Behavioural contract: imaginaire/generators/gancraft_base.py:172-225 (RenderCNN.forward: conv1 1x1 64->256, two residual
 // blocks of two 3x3 convolutions with a style-dependent affine modulation, a residual block of two 1x1 convolutions, conv4
 // 1x1 256->3; LeakyReLU 0.2 throughout) and :588-603 (`_forward_global`: NHWC -> NCHW, denoiser, tanh).
 //
 // The reference runs it per 158x158 tile because the unfused per-pixel stage cannot hold a frame (scenedreamer.py:600-628);
 // its receptive radius is 4 px < pad/2, so evaluating it ONCE on the whole padded frame is the same function of the same
-// pixels (SURVEY.md appendix A "Tiling equivalence").  Every layer is one launch of ONE implicit-GEMM kernel:
+// pixels (DESIGN.md section 1, "Tiling equivalence").  Every layer is one launch of ONE implicit-GEMM kernel:
 //
 //   * activations live in HBM as fp16 hi/lo planes in the operand layout  [plane][row + 1][8-channel chunk][x + 1][8]
 //     (16 B per pixel and chunk, a zero border of one pixel): a 128-pixel row segment of one chunk WITH its halo is one
 //     contiguous 2080-byte range, fetched by one 1-D bulk copy (TMA engine) straight into the K-major, no-swizzle
-//     canonical layout of a tcgen05 operand (rows = pixels, 16 B apart).  A tap (dy, dx) of a 3x3 convolution is the same
+//     canonical layout of a wgmma operand (rows = pixels, 16 B apart).  A tap (dy, dx) of a 3x3 convolution is the same
 //     shared-memory buffer read through another row buffer (dy) and a start address shifted by dx * 16 bytes
-//     (operand form verified on the B200 by sdb_tc_selftest variant 2) -- no im2col, nothing is gathered;
-//   * a CTA owns a tile of 2 image rows x 128 pixels: two fp32 accumulators [128 x 256] = all 512 TMEM columns, so every
-//     16 KB weight stage (one tap x 32 input channels x one fp16 plane, streamed through a 4-stage ring from L2) feeds
-//     8-12 MMAs; input channels go by in double-buffered slabs of 32 (4 row buffers x 4 chunks x hi/lo = 65 KB);
+//     (operand form checked by sdb_tc_selftest variant 2) -- no im2col, nothing is gathered;
+//   * a CTA owns a tile of 2 image rows x 128 pixels; warpgroup o keeps the fp32 accumulators of row o in registers,
+//     [128 pixels x 128 channels] per pass, two passes per tile.  Every 16 KB weight stage (one tap x 32 input channels x
+//     one fp16 plane, streamed through a 4-stage ring from L2) feeds 8-16 MMAs of each warpgroup; input channels go by
+//     in double-buffered slabs of 32 (4 row buffers x 4 chunks x hi/lo = 65 KB);
 //   * fp32-grade arithmetic: fp16 hi/lo split of activations and weights, 3 MMAs per product, fp32 accumulation
 //     (precision 2, the parity mode, like the per-pixel MLP) or one fp16 pass (precision 0 -- the class of the reference's
 //     own default, cuDNN TF32 convolutions);
-//   * epilogue (8 warps, thread = pixel): bias / residual + style modulation / LeakyReLU, split, 16-byte stores that a warp
-//     coalesces into 512 contiguous bytes; the last layer folds conv4 (256 -> 3) and tanh in.
-// Roles: warps 0-7 epilogue, warp 8 activation loader, warp 9 weight loader, warp 10 MMA issuer.
+//   * epilogue on the accumulator fragments (two channels of a pixel per element pair): bias / residual + style
+//     modulation / LeakyReLU, split, 4-byte stores; the last layer folds conv4 (256 -> 3) and tanh in.
+// Roles: warps 0-7 MMA + epilogue (two warpgroups), warp 8 activation loader, warp 9 weight loader.
 // Bound: tensor pipe (5.0 MFLOP per pixel; the activations make one HBM round trip per layer: 0.3 GB of 1.2 TFLOP).
 #include "common.cuh"
 #include "tc05.cuh"
@@ -37,7 +38,8 @@ constexpr uint32_t kChunkRow = kSegH * 16;     // 2080 B: one 8-channel chunk of
 constexpr int kSlabChunks = 4;                 // 32 input channels per slab
 constexpr uint32_t kWStage = 256 * 32 * 2;     // 16 KB: [4 chunks][256 out][8] fp16 of one (slab, tap, plane)
 constexpr int kWStages = 4;
-constexpr int kThreads = 352;
+constexpr int kThreads = 320;
+constexpr int kPasses = 2;                     // output-channel halves per tile (accumulator registers)
 constexpr int kEpiThreads = 256;
 
 enum { EPI_BIAS_LRELU = 0, EPI_RES_MOD_LRELU = 1, EPI_RES_BIAS_LRELU_RGB = 2 };
@@ -88,7 +90,7 @@ __device__ __forceinline__ void unpack8h(uint4 u, float (&v)[8]) {
 }
 
 struct Smem {
-    uint32_t slab[2], wring, bars, tmem_slot, consts, total;
+    uint32_t slab[2], wring, bars, consts, total;
     uint32_t slab_bytes;
 };
 __host__ __device__ inline Smem smem_map(int taps, int planes) {
@@ -101,11 +103,10 @@ __host__ __device__ inline Smem smem_map(int taps, int planes) {
     m.wring = o; o += kWStages * kWStage;
     m.consts = o; o += 6 * kCh * 4 + 64;            // bias | mod_w | mod_b | w4[3][256] | b4
     m.bars = o; o += 16 * 8;
-    m.tmem_slot = o; o += 16;
     m.total = o;
     return m;
 }
-enum { B_SLAB_FULL = 0, B_SLAB_EMPTY = 2, B_W_FULL = 4, B_W_EMPTY = 8, B_ACC_FULL = 12, B_ACC_EMPTY = 13 };
+enum { B_SLAB_FULL = 0, B_SLAB_EMPTY = 2, B_W_FULL = 4, B_W_EMPTY = 8 };
 
 template <bool X3>
 __global__ void __launch_bounds__(kThreads, 1)
@@ -115,7 +116,6 @@ conv_kernel(const LayerParams p)
     constexpr int P = X3 ? 2 : 1;
     const Smem sm = smem_map(p.taps, P);
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem + sm.bars);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(smem + sm.tmem_slot);
     float *sBias = reinterpret_cast<float *>(smem + sm.consts);
     float *sModW = sBias + kCh, *sModB = sModW + kCh, *sW4 = sModB + kCh, *sB4 = sW4 + 3 * kCh;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -133,174 +133,185 @@ conv_kernel(const LayerParams p)
         if (tid < 3) sB4[tid] = p.b4[tid];
     }
     if (tid == 0) {
-        for (int i = 0; i < 2; i++) { tc05::mbar_init(&bars[B_SLAB_FULL + i], 1); tc05::mbar_init(&bars[B_SLAB_EMPTY + i], 1); }
-        for (int i = 0; i < kWStages; i++) { tc05::mbar_init(&bars[B_W_FULL + i], 1); tc05::mbar_init(&bars[B_W_EMPTY + i], 1); }
-        tc05::mbar_init(&bars[B_ACC_FULL], 1);
-        tc05::mbar_init(&bars[B_ACC_EMPTY], kEpiThreads);
+        // the two epilogue warpgroups both read every slab and weight stage: one arrival each frees it
+        for (int i = 0; i < 2; i++) { tc05::mbar_init(&bars[B_SLAB_FULL + i], 1); tc05::mbar_init(&bars[B_SLAB_EMPTY + i], 2); }
+        for (int i = 0; i < kWStages; i++) { tc05::mbar_init(&bars[B_W_FULL + i], 1); tc05::mbar_init(&bars[B_W_EMPTY + i], 2); }
         tc05::fence_mbar_init();
     }
-    if (warp == 8) tc05::tmem_alloc(tmem_slot, 512);
-    tc05::fence_before_thread_sync();
     __syncthreads();
-    tc05::fence_after_thread_sync();
-    const uint32_t tmem = *tmem_slot;
     const size_t in_plane = plane_bytes(p.Hp, p.in_chunks, p.Wp);
 
+    // Every tile is computed in kPasses passes over the input channels, one per 128-wide half of the output channels
+    // (accumulators of a [128 pixel x 128 channel] half: 128 registers per thread of a warpgroup).
     if (warp == 8) {
         // ---------------- activation loader: one slab = rows_in rows x P planes x 4 chunks, 2080 B each ----------------
         uint32_t cnt = 0;
         const int n_copies = rows_in * P * kSlabChunks;
         for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
             const int y0 = (tile / p.tiles_x) * kTileRows, x0 = (tile % p.tiles_x) * kSeg;
-            for (int s = 0; s < n_slabs; s++, cnt++) {
-                const uint32_t buf = cnt & 1u, use = cnt >> 1;
-                if (use > 0) tc05::mbar_wait_backoff(&bars[B_SLAB_EMPTY + buf], (use - 1) & 1u, 64);
-                if (lane == 0) tc05::mbar_arrive_expect_tx(&bars[B_SLAB_FULL + buf], (uint32_t)n_copies * kChunkRow);
-                __syncwarp();
-                for (int i = lane; i < n_copies; i += 32) {
-                    const int c = i % kSlabChunks, pl = (i / kSlabChunks) % P, r = i / (kSlabChunks * P);
-                    const uint8_t *src = p.in + (size_t)pl * in_plane +
-                                         (((size_t)(y0 + row_base + r) * p.in_chunks + s * kSlabChunks + c) * p.Wp + x0) * 16;
-                    tc05::bulk_g2s(smem + sm.slab[buf] + (uint32_t)i * kChunkRow, src, kChunkRow, &bars[B_SLAB_FULL + buf]);
+            for (int pass = 0; pass < kPasses; pass++) {
+                for (int s = 0; s < n_slabs; s++, cnt++) {
+                    const uint32_t buf = cnt & 1u, use = cnt >> 1;
+                    if (use > 0) tc05::mbar_wait_backoff(&bars[B_SLAB_EMPTY + buf], (use - 1) & 1u, 64);
+                    if (lane == 0) tc05::mbar_arrive_expect_tx(&bars[B_SLAB_FULL + buf], (uint32_t)n_copies * kChunkRow);
+                    __syncwarp();
+                    for (int i = lane; i < n_copies; i += 32) {
+                        const int c = i % kSlabChunks, pl = (i / kSlabChunks) % P, r = i / (kSlabChunks * P);
+                        const uint8_t *src = p.in + (size_t)pl * in_plane +
+                                             (((size_t)(y0 + row_base + r) * p.in_chunks + s * kSlabChunks + c) * p.Wp + x0) * 16;
+                        tc05::bulk_g2s(smem + sm.slab[buf] + (uint32_t)i * kChunkRow, src, kChunkRow, &bars[B_SLAB_FULL + buf]);
+                    }
                 }
             }
         }
     } else if (warp == 9) {
-        // ---------------- weight loader: 16 KB stages in (slab, tap, plane) order, the same for every tile ----------------
+        // ---------------- weight loader: 16 KB stages in (slab, tap, plane) order, the same for every tile and pass ----------------
         if (lane == 0) {
             uint32_t cnt = 0;
             for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
                 const int n_stages = n_slabs * taps * P;
-                for (int g = 0; g < n_stages; g++, cnt++) {
-                    const uint32_t st = cnt % kWStages, use = cnt / kWStages;
-                    if (use > 0) tc05::mbar_wait_backoff(&bars[B_W_EMPTY + st], (use - 1) & 1u, 32);
-                    tc05::mbar_arrive_expect_tx(&bars[B_W_FULL + st], kWStage);
-                    tc05::bulk_g2s(smem + sm.wring + st * kWStage, p.wpack + (size_t)g * kWStage, kWStage, &bars[B_W_FULL + st]);
+                for (int pass = 0; pass < kPasses; pass++) {
+                    for (int g = 0; g < n_stages; g++, cnt++) {
+                        const uint32_t st = cnt % kWStages, use = cnt / kWStages;
+                        if (use > 0) tc05::mbar_wait_backoff(&bars[B_W_EMPTY + st], (use - 1) & 1u, 32);
+                        tc05::mbar_arrive_expect_tx(&bars[B_W_FULL + st], kWStage);
+                        tc05::bulk_g2s(smem + sm.wring + st * kWStage, p.wpack + (size_t)g * kWStage, kWStage, &bars[B_W_FULL + st]);
+                    }
                 }
             }
         }
-    } else if (warp == 10) {
-        // ---------------- MMA issuer ----------------
-        if (lane == 0) {
-            const uint32_t idesc = tc05::make_idesc(128, 256, false);
-            uint32_t scnt = 0, wcnt = 0, tcnt = 0;
-            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, tcnt++) {
-                if (tcnt > 0) {
-                    tc05::mbar_wait(&bars[B_ACC_EMPTY], (tcnt - 1) & 1u);
-                    tc05::fence_after_thread_sync();
-                }
-                bool first[kTileRows] = {true, true};
+    } else {
+        // ---------------- MMA + epilogue: warpgroup o = warps 4o .. 4o + 3 owns image row y0 + o ----------------
+        const int o = warp >> 2, t = tid & 127;
+        const size_t out_plane = plane_bytes(p.Hp, kCh / 8, p.Wp);
+        uint32_t scnt = 0, wcnt = 0;
+        for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+            const int y = (tile / p.tiles_x) * kTileRows + o, x0 = (tile % p.tiles_x) * kSeg;
+            // rgb partial sums of the 4 pixels this thread holds fragments of: [row block][+8][channel]
+            float rgb[2][2][3];
+#pragma unroll
+            for (int i = 0; i < 12; i++) (&rgb[0][0][0])[i] = 0.0f;
+#pragma unroll 1
+            for (int pass = 0; pass < kPasses; pass++) {
+                // acc[rb][nh]: pixels 64 rb .., output channels 128 pass + 64 nh ..
+                float acc[2][2][32];
+#pragma unroll
+                for (int i = 0; i < 128; i++) (&acc[0][0][0])[i] = 0.0f;
                 for (int s = 0; s < n_slabs; s++, scnt++) {
                     const uint32_t buf = scnt & 1u;
                     tc05::mbar_wait(&bars[B_SLAB_FULL + buf], (scnt >> 1) & 1u);
-                    tc05::fence_after_thread_sync();
                     const uint32_t slab = tc05::smem_u32(smem + sm.slab[buf]);
-                    for (int t = 0; t < taps; t++) {
-                        const int dy = taps == 9 ? t / 3 : 0, dx = taps == 9 ? t % 3 : 1;
+                    for (int tp = 0; tp < taps; tp++) {
+                        const int dy = taps == 9 ? tp / 3 : 0, dx = taps == 9 ? tp % 3 : 1;
 #pragma unroll
                         for (int pw = 0; pw < P; pw++, wcnt++) {
                             const uint32_t st = wcnt % kWStages;
                             tc05::mbar_wait(&bars[B_W_FULL + st], (wcnt / kWStages) & 1u);
-                            tc05::fence_after_thread_sync();
-                            const uint32_t wbase = tc05::smem_u32(smem + sm.wring + st * kWStage);
+                            const uint32_t wbase = tc05::smem_u32(smem + sm.wring + st * kWStage) + (uint32_t)pass * 128u * 16u;
                             // products with this weight plane: W_hi meets A_hi and (x3) A_lo; W_lo meets A_hi only
                             const int n_pa = (X3 && pw == 0) ? 2 : 1;
+                            tc05::wgmma_fence();
+                            for (int pa = 0; pa < n_pa; pa++) {
 #pragma unroll
-                            for (int o = 0; o < kTileRows; o++) {
-                                for (int pa = 0; pa < n_pa; pa++) {
+                                for (int k16 = 0; k16 < 2; k16++) {
+                                    const uint32_t a_addr = slab + (uint32_t)(((o + dy) * P + pa) * kSlabChunks + 2 * k16) * kChunkRow + dx * 16;
 #pragma unroll
-                                    for (int k16 = 0; k16 < 2; k16++) {
-                                        const uint32_t a_addr = slab + (uint32_t)(((o + dy) * P + pa) * kSlabChunks + 2 * k16) * kChunkRow + dx * 16;
-                                        const uint64_t da = tc05::make_smem_desc(a_addr, kChunkRow, 128);
-                                        const uint64_t db = tc05::make_smem_desc(wbase + (uint32_t)(2 * k16) * 4096u, 4096u, 128);
-                                        tc05::mma_f16_ss(tmem + (uint32_t)o * 256u, da, db, idesc, first[o] ? 0u : 1u);
-                                        first[o] = false;
+                                    for (int rb = 0; rb < 2; rb++) {
+                                        const uint64_t da = tc05::make_smem_desc(a_addr + rb * 1024u, kChunkRow, 128);
+#pragma unroll
+                                        for (int nh = 0; nh < 2; nh++) {
+                                            const uint64_t db = tc05::make_smem_desc(wbase + (uint32_t)(2 * k16) * 4096u + nh * 1024u, 4096u, 128);
+                                            tc05::wgmma_m64n64k16<false, 0, 0>(acc[rb][nh], da, db, 1u);
+                                        }
                                     }
                                 }
                             }
-                            tc05::mma_commit(&bars[B_W_EMPTY + st]);
+                            tc05::wgmma_commit();
+                            tc05::wgmma_wait<0>();
+#pragma unroll
+                            for (int rb = 0; rb < 2; rb++)
+#pragma unroll
+                                for (int nh = 0; nh < 2; nh++) tc05::wgmma_fence_acc(acc[rb][nh]);
+                            tc05::named_sync(1 + o, 128);
+                            if (t == 0) tc05::mbar_arrive(&bars[B_W_EMPTY + st]);
                         }
                     }
-                    tc05::mma_commit(&bars[B_SLAB_EMPTY + buf]);
+                    if (t == 0) tc05::mbar_arrive(&bars[B_SLAB_EMPTY + buf]);
                 }
-                tc05::mma_commit(&bars[B_ACC_FULL]);
-            }
-        }
-    } else {
-        // ---------------- epilogue: warps 0-3 own image row y0, warps 4-7 row y0 + 1; thread = pixel ----------------
-        const int o = warp >> 2, row = (warp & 3) * 32 + lane;
-        const uint32_t tm_row = tmem + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)o * 256u;
-        const size_t out_plane = plane_bytes(p.Hp, kCh / 8, p.Wp);
-        uint32_t tcnt = 0;
-        for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, tcnt++) {
-            const int y = (tile / p.tiles_x) * kTileRows + o, x = (tile % p.tiles_x) * kSeg + row;
-            const bool valid = y < p.H && x < p.W;
-            tc05::mbar_wait(&bars[B_ACC_FULL], tcnt & 1u);
-            tc05::fence_after_thread_sync();
-            // element offset of (pixel, chunk 0) inside a 256-channel plane
-            const size_t pix = (((size_t)(y + 1) * (kCh / 8)) * p.Wp + (x + 1)) * 16;
-            float rgb[3] = {0.0f, 0.0f, 0.0f};
-#pragma unroll 1
-            for (int c0 = 0; c0 < kCh; c0 += 16) {
-                float v[16];
-                tc05::tmem_ld16(tm_row + c0, v);
-                tc05::tmem_ld_wait();
+                // ---- epilogue of this channel half, on the accumulator fragments: element (pixel, c, c + 1) per pair ----
 #pragma unroll
-                for (int q = 0; q < 2; q++) {
-                    float(&v8)[8] = *reinterpret_cast<float(*)[8]>(&v[8 * q]);
-                    const int ch0 = c0 + 8 * q;
-                    const size_t off = pix + (size_t)(ch0 >> 3) * p.Wp * 16;
-                    if (p.epi != EPI_BIAS_LRELU) {
-                        float r8[8];
-                        unpack8h(__ldg(reinterpret_cast<const uint4 *>(p.res + off)), r8);
-                        if (X3) {
-                            float l8[8];
-                            unpack8h(__ldg(reinterpret_cast<const uint4 *>(p.res + out_plane + off)), l8);
+                for (int rb = 0; rb < 2; rb++) {
 #pragma unroll
-                            for (int j = 0; j < 8; j++) r8[j] += l8[j];
+                    for (int h = 0; h < 2; h++) {
+                        const int px = rb * 64 + tc05::frag_row(t, 2 * h), x = x0 + px;
+                        const bool valid = y < p.H && x < p.W;
+                        const size_t pix = (((size_t)(y + 1) * (kCh / 8)) * p.Wp + (x + 1)) * 16;
+#pragma unroll
+                        for (int nh = 0; nh < 2; nh++) {
+#pragma unroll
+                            for (int j = 0; j < 8; j++) {
+                                const int ch = pass * 128 + nh * 64 + tc05::frag_col(t, 4 * j);
+                                float v0 = acc[rb][nh][4 * j + 2 * h], v1 = acc[rb][nh][4 * j + 2 * h + 1];
+                                const size_t off = pix + (size_t)(ch >> 3) * p.Wp * 16 + (ch & 7) * 2;
+                                if (p.epi != EPI_BIAS_LRELU) {
+                                    float2 r = __half22float2(*reinterpret_cast<const __half2 *>(p.res + off));
+                                    if (X3) {
+                                        const float2 l = __half22float2(*reinterpret_cast<const __half2 *>(p.res + out_plane + off));
+                                        r.x += l.x;
+                                        r.y += l.y;
+                                    }
+                                    v0 = r.x + v0;                                            // y + conv(...)
+                                    v1 = r.y + v1;
+                                }
+                                if (p.epi == EPI_RES_MOD_LRELU) {
+                                    v0 = lrelu(fmaf(v0, sModW[ch], sModB[ch]));
+                                    v1 = lrelu(fmaf(v1, sModW[ch + 1], sModB[ch + 1]));
+                                } else if (p.epi == EPI_RES_BIAS_LRELU_RGB) {
+                                    v0 = lrelu(v0 + sBias[ch]);
+                                    v1 = lrelu(v1 + sBias[ch + 1]);
+#pragma unroll
+                                    for (int k = 0; k < 3; k++)
+                                        rgb[rb][h][k] = fmaf(v1, sW4[k * kCh + ch + 1], fmaf(v0, sW4[k * kCh + ch], rgb[rb][h][k]));
+                                } else {
+                                    v0 = lrelu(v0 + sBias[ch]);
+                                    v1 = lrelu(v1 + sBias[ch + 1]);
+                                }
+                                if (p.out != nullptr && valid) {
+                                    const __half2 hi = __floats2half2_rn(v0, v1);
+                                    *reinterpret_cast<__half2 *>(p.out + off) = hi;
+                                    if (X3) {
+                                        const float2 back = __half22float2(hi);
+                                        *reinterpret_cast<__half2 *>(p.out + out_plane + off) = __floats2half2_rn(v0 - back.x, v1 - back.y);
+                                    }
+                                }
+                            }
                         }
-#pragma unroll
-                        for (int j = 0; j < 8; j++) v8[j] = r8[j] + v8[j];                         // y + conv(...)
-                    }
-                    if (p.epi == EPI_RES_MOD_LRELU) {
-#pragma unroll
-                        for (int j = 0; j < 8; j++) v8[j] = lrelu(fmaf(v8[j], sModW[ch0 + j], sModB[ch0 + j]));
-                    } else if (p.epi == EPI_RES_BIAS_LRELU_RGB) {
-#pragma unroll
-                        for (int j = 0; j < 8; j++) {
-                            v8[j] = lrelu(v8[j] + sBias[ch0 + j]);
-                            rgb[0] = fmaf(v8[j], sW4[ch0 + j], rgb[0]);
-                            rgb[1] = fmaf(v8[j], sW4[kCh + ch0 + j], rgb[1]);
-                            rgb[2] = fmaf(v8[j], sW4[2 * kCh + ch0 + j], rgb[2]);
-                        }
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 8; j++) v8[j] = lrelu(v8[j] + sBias[ch0 + j]);
-                    }
-                    if (p.out != nullptr && valid) {
-                        uint4 hi, lo;
-                        split8h(v8, hi, lo);
-                        *reinterpret_cast<uint4 *>(p.out + off) = hi;
-                        if (X3) *reinterpret_cast<uint4 *>(p.out + out_plane + off) = lo;
                     }
                 }
             }
-            tc05::fence_before_thread_sync();
-            tc05::mbar_arrive(&bars[B_ACC_EMPTY]);
-            if (p.epi == EPI_RES_BIAS_LRELU_RGB && valid) {
+            if (p.epi == EPI_RES_BIAS_LRELU_RGB) {
+                // the 4 threads of a quad hold the same pixels: sum their channel partials, one of them writes
 #pragma unroll
-                for (int k = 0; k < 3; k++) {
-                    const float raw = rgb[k] + sB4[k];
-                    const size_t idx = ((size_t)k * p.H + y) * p.W + x;
-                    p.rgb[idx] = tanhf(raw);
-                    if (p.rgb_raw) p.rgb_raw[idx] = raw;
-                }
+                for (int rb = 0; rb < 2; rb++)
+#pragma unroll
+                    for (int h = 0; h < 2; h++) {
+                        const int x = x0 + rb * 64 + tc05::frag_row(t, 2 * h);
+#pragma unroll
+                        for (int k = 0; k < 3; k++) {
+                            float v = rgb[rb][h][k];
+                            v += __shfl_xor_sync(0xffffffffu, v, 1);
+                            v += __shfl_xor_sync(0xffffffffu, v, 2);
+                            if ((lane & 3) == 0 && y < p.H && x < p.W) {
+                                const float raw = v + sB4[k];
+                                const size_t idx = ((size_t)k * p.H + y) * p.W + x;
+                                p.rgb[idx] = tanhf(raw);
+                                if (p.rgb_raw) p.rgb_raw[idx] = raw;
+                            }
+                        }
+                    }
             }
         }
     }
-    tc05::fence_before_thread_sync();
-    __syncthreads();
-    if (warp == 8) tc05::tmem_dealloc(tmem, 512);
 }
 
 // per-pixel features fp32 [H][W][64] (NHWC, the fused kernel's net_out) -> operand planes [P][Hp][8][Wp][8] fp16

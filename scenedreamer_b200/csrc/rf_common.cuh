@@ -16,8 +16,8 @@ constexpr int kKH = kHidden + kKExt;            // 272: K of every forward layer
 constexpr int kMaxM = 8, kMaxS = 64, kMaxLabels = 15;
 constexpr int kEpiThreads = 256, kGatherThreads = 256;
 // warpgroup-aligned roles so that setmaxnreg can move registers from the control group to the gather group:
-//   WG0-1 epilogue (warps 0-7), WG2 control (8: weight loader, 9: MMA issuer, 10-11 idle), WG3-4 gather (12-19)
-constexpr int kLoaderWarp = 8, kMmaWarp = 9, kGatherWarp0 = 12;
+//   WG0-1 epilogue (warps 0-7), WG2 MMA + weight loads (warps 8-11), WG3-4 gather (12-19)
+constexpr int kMmaWarp0 = 8, kGatherWarp0 = 12;
 constexpr int kThreads = kEpiThreads + 128 + kGatherThreads;   // 640
 // setmaxnreg can only redistribute the registers the CTA was LAUNCHED with (640 threads x 96 = 61,440; the
 // allocator is a per-CTA pool -- USETMAXREG.TRY_ALLOC.CTAPOOL spins forever otherwise):
@@ -26,7 +26,6 @@ constexpr int kRegsLaunch = 96, kRegsCtl = 48, kRegsGather = 120;
 static_assert(8 * 32 * kRegsLaunch + 4 * 32 * kRegsCtl + 8 * 32 * kRegsGather <= kThreads * kRegsLaunch,
               "setmaxnreg budget exceeds the CTA's launch-time register allocation");
 constexpr int kRingBytes = 65536;
-constexpr uint32_t kTmemCols = 512;
 constexpr uint32_t kLboA = kRows * 16, kSbo = 128;
 constexpr int kHChunks = kKH / 8;               // 34 16-byte k-chunks per row
 constexpr int kHBytes = kHChunks * kRows * 16;  // 69,632 bytes per operand part
@@ -113,7 +112,7 @@ __device__ __forceinline__ bool elect_one() {
 
 // ---- shared memory map ---------------------------------------------------------------------------
 struct Smem {
-    uint32_t h_hi, h_lo, ring, fsec, scales, frac, sig, state, bars, tmem_slot, stop, sched, total;
+    uint32_t h_hi, h_lo, ring, fsec, scales, frac, sig, state, bars, stop, sched, total;
 };
 __host__ __device__ constexpr Smem smem_map(bool x3) {
     Smem m{};
@@ -127,7 +126,6 @@ __host__ __device__ constexpr Smem smem_map(bool x3) {
     m.sig = o; o += 2 * kRows * 4;
     m.state = o; o += 2 * (2 * kMaxM + 6) * kRows * 4;
     m.bars = o; o += 40 * 8;
-    m.tmem_slot = o; o += 16;
     m.stop = o; o += 16;                         // early termination: int stop_step[2] (per tile buffer), int vote[2]
     m.sched = o; o += 32;                        // dynamic tile scheduler: int work[4] (ring), int published
     m.total = o;
@@ -159,7 +157,7 @@ constexpr int kNumAct = 6;
 //   [work item = slot / 128][chunk = column / 8][row = slot % 128][8 columns]      (16 B per (row, chunk), 2 KB per chunk)
 // so that (a) a warp of 32 consecutive rows writes 512 contiguous bytes per store instruction and (b) one item of an
 // array is a contiguous range that the weight-gradient kernel (wgrad.cu) bulk-copies into shared memory, where it is a
-// canonical MN-major tcgen05 operand whose reduction dimension is the samples.
+// canonical MN-major wgmma operand whose reduction dimension is the samples.
 __host__ __device__ __forceinline__ uint16_t *rec_chunk(uint16_t *base, long long slot, int n_chunks, int chunk) {
     return base + ((((slot >> 7) * n_chunks + chunk) << 10) + ((slot & 127) << 3));
 }
@@ -214,7 +212,26 @@ struct Params {
     float *sky_partial;            // [n_tiles, 64] per-tile column sums (deterministic mean)
     int32_t *debug;                // optional host-mapped progress buffer (diagnostics), else nullptr
     TrainBuf tr;                   // training record (TRAIN forward writes it, the kBwd chain reads it)
+    float *acc;                    // [grid][2][128][256] fp32 accumulator buffers, set by the launcher
 };
+
+// NV consecutive fp32 accumulators of one row (written by the MMA warpgroup of the same CTA: plain loads, not the
+// non-coherent path)
+// SDB_AB_NO_ACC (diagnostics build only, results are wrong): the accumulator buffer is neither written nor read, so that
+// the kernel time with and without that traffic can be compared on the same work (bench.py --no-early-stop).
+template <int NV>
+__device__ __forceinline__ void acc_ld(const float *src, float (&v)[NV]) {
+#ifdef SDB_AB_NO_ACC
+#pragma unroll
+    for (int i = 0; i < NV; i++) v[i] = __int_as_float((int)(reinterpret_cast<uintptr_t>(src) & 1));   // 0.0f, not a constant
+    return;
+#endif
+#pragma unroll
+    for (int i = 0; i < NV; i += 4) {
+        const float4 a = *reinterpret_cast<const float4 *>(src + i);
+        v[i] = a.x; v[i + 1] = a.y; v[i + 2] = a.z; v[i + 3] = a.w;
+    }
+}
 
 // progress markers (CTA 0 only): debug[role*4 + {0,1,2}] = {marker, step, layer/stage}
 #define SDB_MARK(role, marker, a, b)                                              \
@@ -227,7 +244,7 @@ struct Params {
 
 // timeline of CTA 0 (diagnostics, tools/render_timeline.py; library built with SDB_NVCC_EXTRA=-DSDB_TIMELINE): with debug[60] == kTraceMagic, sample steps
 // debug[61] .. debug[61]+kTraceSteps-1 of the CTA record clock() stamps, debug[64 + ((n - first) * 8 + layer) * 8 + slot]:
-//   slot 0 issuer: operands of the layer's first stage may be waited for   1 issuer: last MMA of the layer issued
+//   slot 0 MMA warpgroup: the layer's inputs are ready (buffer free, operand written)   1 MMA warpgroup: the layer's accumulators are written
 //   slot 2/4 epilogue half 0/1: accumulator of the layer complete          3/5 epilogue half 0/1: last slab handed over
 //   layer row 7 = the gather role preparing step n: 0 compositing of step n-2 seen, 1 slots refilled, 2 features gathered, 3 operand buffer free
 constexpr int32_t kTraceMagic = 0x7131;
@@ -257,18 +274,14 @@ __device__ __forceinline__ TileCoord tile_coord(const Params &p, int tile) {
     return t;
 }
 
-// 256-bit global store (STG.256): a thread's 32 contiguous bytes in ONE instruction -- the per-row record writes of
-// the training kernels touch 32 different lines per warp instruction, so halving the instruction count halves the
-// LSU work.  `p` must be 32-byte aligned.
+// a thread's 32 contiguous bytes as two 128-bit global stores (`p` 32-byte aligned)
 __device__ __forceinline__ void st_global_v8(void *p, uint4 a, uint4 b) {
-    asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w),
-                 "r"(b.x), "r"(b.y), "r"(b.z), "r"(b.w)
-                 : "memory");
+    reinterpret_cast<uint4 *>(p)[0] = a;
+    reinterpret_cast<uint4 *>(p)[1] = b;
 }
 __device__ __forceinline__ void st_global_v8f(float *p, const float *v) {
-    asm volatile("st.global.v8.f32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]),
-                 "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7])
-                 : "memory");
+    reinterpret_cast<float4 *>(p)[0] = make_float4(v[0], v[1], v[2], v[3]);
+    reinterpret_cast<float4 *>(p)[1] = make_float4(v[4], v[5], v[6], v[7]);
 }
 
 __device__ __forceinline__ void ld8(const float *g, float (&v)[8]) {

@@ -1,6 +1,6 @@
-// Thin inline-PTX layer over the Blackwell (sm_100a) tensor-core path used by the fused render
-// kernel: tcgen05.mma (kind::f16, operands in shared memory, fp32 accumulators in TMEM), TMEM
-// allocation / loads, mbarriers, bulk async copies (TMA 1-D) and the proxy fences between them.
+// Thin inline-PTX layer over the Hopper (sm_90a) tensor-core path used by the fused kernels:
+// wgmma.mma_async (operands in shared memory, fp32 accumulators in the registers of a warpgroup),
+// mbarriers, bulk async copies (TMA 1-D) and the proxy fences between them.
 //
 // Operand layout (both A and B are K-major, SWIZZLE_NONE "interleaved" canonical layout):
 //   the matrix is cut into 8-row x 16-byte core matrices, each stored as 128 contiguous bytes;
@@ -11,6 +11,8 @@
 //   thread that owns row r writes its 8 consecutive k-values with ONE 16-byte st.shared and a
 //   warp (32 consecutive rows) writes 512 contiguous bytes -> conflict-free epilogue stores, and
 //   a weight K-chunk is one contiguous range that a single cp.async.bulk can fetch.
+// The same canonical layout is a wgmma operand (SWIZZLE_NONE descriptors), so the data formats of
+// the kernels are independent of which tensor-core generation consumes them.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -23,86 +25,85 @@ __device__ __forceinline__ uint32_t smem_u32(const void *p) {
 }
 
 // ---- descriptors -----------------------------------------------------------------------------
-// 64-bit shared-memory matrix descriptor (SWIZZLE_NONE, version 1 = Blackwell):
-//   [0,14) start address >> 4, [16,30) LBO >> 4, [32,46) SBO >> 4, [46,48) version, [61,64) layout.
+// 64-bit shared-memory matrix descriptor of wgmma (layout type 0 = no swizzle, base offset 0):
+//   [0,14) start address >> 4, [16,30) LBO >> 4, [32,46) SBO >> 4.
+// K-major operands: LBO = distance of the two 8-element K core matrices, SBO = distance of 8-row groups.
+// MN-major operands: LBO = distance of 8-sample (K) groups, SBO = distance of 8-element MN groups.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
     return d;
 }
 
-// 32-bit instruction descriptor for kind::f16 with fp32 accumulation, both operands K-major:
-//   [4,6) D format (1 = f32), [7,10) A format, [10,13) B format (0 = f16, 1 = bf16),
-//   [15] A major (0 = K), [16] B major (0 = K), [17,23) N >> 3, [24,29) M >> 4.
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t M, uint32_t N, bool bf16) {
-    return (1u << 4) | ((bf16 ? 1u : 0u) << 7) | ((bf16 ? 1u : 0u) << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
+// ---- warpgroup MMA (sm_90a wgmma) -------------------------------------------------------------------
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, both operands in shared memory, fp32 accumulators in the registers of the
+// 128 threads of the issuing warpgroup (all of them execute it).  TA / TB = 1: the operand is MN-major (transposed).
+// Accumulator fragment: thread t = 32 w + l holds d[4 j + 2 h + e] = D[16 w + l / 4 + 8 h][8 j + 2 (l % 4) + e].
+template <bool BF16, int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n16k16(float (&d)[8], uint64_t da, uint64_t db, uint32_t accumulate) {
+    if constexpr (BF16)
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t}\n"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+                     : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+    else
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t}\n"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+                     : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
 }
 
-// ---- MMA issue / completion --------------------------------------------------------------------
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread on behalf of the CTA.
-__device__ __forceinline__ void mma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                           uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
+template <bool BF16, int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
+    if constexpr (BF16)
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}\n"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                     : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+    else
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}\n"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                     : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
 }
 
-// Make the mbarrier track completion of all MMAs issued so far by this thread (implies
-// tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void mma_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
+template <bool BF16, int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+    if constexpr (BF16)
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}\n"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                     : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+    else
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}\n"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                     : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
 }
 
-__device__ __forceinline__ void fence_before_thread_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_thread_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int R>
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
+}
 // generic-proxy smem writes -> visible to the async proxy (tensor core / TMA reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ---- TMEM --------------------------------------------------------------------------------------
-// One full warp allocates `cols` (power of two >= 32) columns; the base address lands in *slot.
-__device__ __forceinline__ void tmem_alloc(uint32_t *slot_smem, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_smem)), "r"(cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
+// named barrier over the `threads` threads that use barrier `id` (1..15)
+__device__ __forceinline__ void named_sync(uint32_t id, uint32_t threads) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp gets row (lane base + i).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-    uint32_t *r = reinterpret_cast<uint32_t *>(v);
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-// 32 lanes x 16 consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t *r = reinterpret_cast<uint32_t *>(v);
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// fragment row / column of accumulator element i of thread `t` of a warpgroup (see the layout above)
+__device__ __forceinline__ int frag_row(int t, int i) { return ((t >> 5) << 4) + ((t & 31) >> 2) + (((i >> 1) & 1) << 3); }
+__device__ __forceinline__ int frag_col(int t, int i) { return ((i >> 2) << 3) + ((t & 3) << 1) + (i & 1); }
 
 // ---- mbarrier ----------------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {

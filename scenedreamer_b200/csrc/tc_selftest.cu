@@ -1,6 +1,6 @@
-// tcgen05 / TMEM self test: C[128, N] = A[128, K] * B[N, K]^T (fp32 accumulate) through exactly the
-// shared-memory descriptors, instruction descriptor, commit/mbarrier and TMEM load paths that the
-// fused render kernel uses (tc05.cuh).  Used by tests/ to validate the operand layout on hardware.
+// Tensor-core self test: C[128, N] = A[128, K] * B[N, K]^T (fp32 accumulate) through exactly the
+// shared-memory operand layouts and descriptors that the fused kernels use with wgmma (tc05.cuh).
+// Used by tests/ to validate the operand layout on hardware.
 #include "common.cuh"
 #include "tc05.cuh"
 
@@ -14,9 +14,7 @@ tc_selftest_kernel(const float *__restrict__ a, const float *__restrict__ b, flo
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t *sA = smem;
     uint8_t *sB = smem + 130 * K * 2;
-    uint64_t *bar = reinterpret_cast<uint64_t *>(sB + N * K * 2);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bar + 1);
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x;
 
     const int KC = K / 8;
     // variant 2 (layout of the convolution kernel, rendercnn.cu): A holds 130 rows per 8-column chunk -- a pixel row with a
@@ -45,52 +43,36 @@ tc_selftest_kernel(const float *__restrict__ a, const float *__restrict__ b, flo
         v.w = tc05::pack2<BF16>(src[6], src[7]);
         *reinterpret_cast<uint4 *>(sB + tc05::chunk_off(N, r, kc)) = v;
     }
-    uint32_t cols = 32;
-    while ((int)cols < N) cols <<= 1;
-    if (tid == 0) {
-        tc05::mbar_init(bar, 1);
-        tc05::fence_mbar_init();
-    }
-    if (warp == 0) tc05::tmem_alloc(tmem_slot, cols);
     tc05::fence_proxy_async_smem();
-    tc05::fence_before_thread_sync();
     __syncthreads();
-    tc05::fence_after_thread_sync();
-    const uint32_t tmem = *tmem_slot;
 
-    if (tid == 0) {
-        const uint32_t idesc = tc05::make_idesc(128, N, BF16);
-        const uint32_t lboA = 128 * 16, lboB = N * 16, sbo = 128;
-        for (int kk = 0; kk < K / 16; kk++) {
-            uint64_t da, db;
-            if (variant == 2) {
-                da = tc05::make_smem_desc(tc05::smem_u32(sA) + 16 + kk * 2 * 130 * 16, 130 * 16, sbo);
-                db = tc05::make_smem_desc(tc05::smem_u32(sB) + kk * 2 * lboB, lboB, sbo);
-            } else if (variant == 0) {
-                da = tc05::make_smem_desc(tc05::smem_u32(sA) + kk * 2 * lboA, lboA, sbo);
-                db = tc05::make_smem_desc(tc05::smem_u32(sB) + kk * 2 * lboB, lboB, sbo);
-            } else {  // LBO / SBO meaning swapped (diagnostic)
-                da = tc05::make_smem_desc(tc05::smem_u32(sA) + kk * 2 * lboA, sbo, lboA);
-                db = tc05::make_smem_desc(tc05::smem_u32(sB) + kk * 2 * lboB, sbo, lboB);
+    // one warpgroup: two 64-row blocks x 16-column slices of C, K in 16-wide steps
+    const uint32_t lboA = (variant == 2 ? 130 : 128) * 16, lboB = N * 16, sbo = 128;
+    for (int rb = 0; rb < 2; rb++) {
+        for (int n0 = 0; n0 < N; n0 += 16) {
+            float d[8];
+            for (int kk = 0; kk < K / 16; kk++) {
+                const uint32_t a0 = tc05::smem_u32(sA) + (variant == 2 ? 16u : 0u) + kk * 2 * lboA + rb * 1024;
+                const uint32_t b0 = tc05::smem_u32(sB) + kk * 2 * lboB + n0 * 16;
+                uint64_t da, db;
+                if (variant == 1) {      // LBO / SBO meaning swapped (diagnostic)
+                    da = tc05::make_smem_desc(a0, sbo, lboA);
+                    db = tc05::make_smem_desc(b0, sbo, lboB);
+                } else {
+                    da = tc05::make_smem_desc(a0, lboA, sbo);
+                    db = tc05::make_smem_desc(b0, lboB, sbo);
+                }
+                tc05::wgmma_fence();
+                tc05::wgmma_m64n16k16<BF16, 0, 0>(d, da, db, kk > 0 ? 1u : 0u);
+                tc05::wgmma_commit();
+                tc05::wgmma_wait<0>();
+                tc05::wgmma_fence_acc(d);
             }
-            tc05::mma_f16_ss(tmem, da, db, idesc, kk > 0 ? 1u : 0u);
-        }
-        tc05::mma_commit(bar);
-    }
-    tc05::mbar_wait(bar, 0);
-    tc05::fence_after_thread_sync();
-    const int row = tid;
-    for (int c0 = 0; c0 < N; c0 += 32) {
-        float v[32];
-        tc05::tmem_ld32(tmem + ((uint32_t)(warp * 32) << 16) + c0, v);
-        tc05::tmem_ld_wait();
 #pragma unroll
-        for (int j = 0; j < 32; j++)
-            if (c0 + j < N) c[(size_t)row * N + c0 + j] = v[j];
+            for (int i = 0; i < 8; i++)
+                c[(size_t)(rb * 64 + tc05::frag_row(tid, i)) * N + n0 + tc05::frag_col(tid, i)] = d[i];
+        }
     }
-    tc05::fence_before_thread_sync();
-    __syncthreads();
-    if (warp == 0) tc05::tmem_dealloc(tmem, cols);
 }
 
 }  // namespace
@@ -116,7 +98,7 @@ extern "C" int sdb_tc_selftest(const float *d_a, const float *d_b, float *d_c, i
 // ---- MN-major operands (diagnostic for the planned weight-gradient kernel) ---------------------------------------------
 // C[F=128, G] = X^T Y with X [S=128 samples, 128], Y [S=128, G]: the SAMPLES are the reduction dimension, and X / Y sit in
 // shared memory exactly as the fused kernels keep activations: [feature chunk of 8][128 sample rows][8 features] (16 B per
-// row).  Read as an MMA operand with M (or N) = features and K = samples this is an MN-major canonical layout: 8 features
+// row), read by wgmma with both operands transposed (MN-major).  Read as an MMA operand with M (or N) = features and K = samples this is an MN-major canonical layout: 8 features
 // contiguous, the 8 samples of a core matrix 16 B apart, next 8 samples +128 B, next 8 features +2048 B.
 // variant 0: LBO = 128 (K direction), SBO = 2048 (MN direction); variant 1: swapped.
 namespace {
@@ -126,9 +108,7 @@ tc_selftest_mn_kernel(const float *__restrict__ x, const float *__restrict__ y, 
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t *sX = smem;
     uint8_t *sY = smem + 128 * 128 * 2;
-    uint64_t *bar = reinterpret_cast<uint64_t *>(sY + 128 * G * 2);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bar + 1);
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x;
     for (int i = tid; i < 128 * 16; i += 128) {           // X: 128 samples x 16 feature chunks
         const int r = i / 16, kc = i % 16;
         const float *src = x + (size_t)r * 128 + kc * 8;
@@ -143,42 +123,27 @@ tc_selftest_mn_kernel(const float *__restrict__ x, const float *__restrict__ y, 
             make_uint4(tc05::pack2<true>(src[0], src[1]), tc05::pack2<true>(src[2], src[3]), tc05::pack2<true>(src[4], src[5]),
                        tc05::pack2<true>(src[6], src[7]));
     }
-    uint32_t cols = 32;
-    while ((int)cols < G) cols <<= 1;
-    if (tid == 0) {
-        tc05::mbar_init(bar, 1);
-        tc05::fence_mbar_init();
-    }
-    if (warp == 0) tc05::tmem_alloc(tmem_slot, cols);
     tc05::fence_proxy_async_smem();
-    tc05::fence_before_thread_sync();
     __syncthreads();
-    tc05::fence_after_thread_sync();
-    const uint32_t tmem = *tmem_slot;
-    if (tid == 0) {
-        const uint32_t idesc = tc05::make_idesc(128, G, true) | (1u << 15) | (1u << 16);       // A and B MN-major
-        const uint32_t kdir = 128, mndir = 128 * 16;
-        for (int kk = 0; kk < 8; kk++) {                  // 16 samples per MMA
-            const uint32_t lbo = variant == 0 ? kdir : mndir, sbo = variant == 0 ? mndir : kdir;
-            const uint64_t da = tc05::make_smem_desc(tc05::smem_u32(sX) + kk * 256, lbo, sbo);
-            const uint64_t db = tc05::make_smem_desc(tc05::smem_u32(sY) + kk * 256, lbo, sbo);
-            tc05::mma_f16_ss(tmem, da, db, idesc, kk > 0 ? 1u : 0u);
-        }
-        tc05::mma_commit(bar);
-    }
-    tc05::mbar_wait(bar, 0);
-    tc05::fence_after_thread_sync();
-    for (int c0 = 0; c0 < G; c0 += 32) {
-        float v[32];
-        tc05::tmem_ld32(tmem + ((uint32_t)(warp * 32) << 16) + c0, v);
-        tc05::tmem_ld_wait();
+    const uint32_t kdir = 128, mndir = 128 * 16;
+    const uint32_t lbo = variant == 0 ? kdir : mndir, sbo = variant == 0 ? mndir : kdir;
+    for (int rb = 0; rb < 2; rb++) {                       // features 64 rb .. 64 rb + 63 = 8 chunks of 8
+        for (int n0 = 0; n0 < G; n0 += 16) {
+            float d[8];
+            for (int kk = 0; kk < 8; kk++) {              // 16 samples per MMA
+                const uint64_t da = tc05::make_smem_desc(tc05::smem_u32(sX) + rb * 8 * mndir + kk * 256, lbo, sbo);
+                const uint64_t db = tc05::make_smem_desc(tc05::smem_u32(sY) + (n0 / 8) * mndir + kk * 256, lbo, sbo);
+                tc05::wgmma_fence();
+                tc05::wgmma_m64n16k16<true, 1, 1>(d, da, db, kk > 0 ? 1u : 0u);
+                tc05::wgmma_commit();
+                tc05::wgmma_wait<0>();
+                tc05::wgmma_fence_acc(d);
+            }
 #pragma unroll
-        for (int j = 0; j < 32; j++)
-            if (c0 + j < G) c[(size_t)tid * G + c0 + j] = v[j];
+            for (int i = 0; i < 8; i++)
+                c[(size_t)(rb * 64 + tc05::frag_row(tid, i)) * G + n0 + tc05::frag_col(tid, i)] = d[i];
+        }
     }
-    tc05::fence_before_thread_sync();
-    __syncthreads();
-    if (warp == 0) tc05::tmem_dealloc(tmem, cols);
 }
 }  // namespace
 

@@ -1,4 +1,4 @@
-// f3 (SURVEY.md 8(f)-3): building the voxel world of a scene from its bird's-eye-view maps ON THE DEVICE.
+// f3: building the voxel world of a scene from its bird's-eye-view maps ON THE DEVICE.
 // Behavioural contract: PCGVoxelGenerator.next_world (imaginaire/model_utils/pcg_gen.py:83-174):
 //   world[h, x, z] = label(x, z) for h = hq(x, z) and for clip(hq + 1 .. hq + 16, 0, 255)        (:119-125, surface shell, hollow below)
 //   trees: voxel models pasted at height hq + 16 in iteration order, only where the world is still 0 (:132-151);

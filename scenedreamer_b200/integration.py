@@ -1,4 +1,4 @@
-"""Reference-side integration: SceneDreamer's `Generator` on the fused B200 kernels, with ZERO edits to the reference.
+"""Reference-side integration: SceneDreamer's `Generator` on the fused H100 kernels, with ZERO edits to the reference.
 
 How the hook gets in.  The reference's `imaginaire/generators/scenedreamer.py:13` imports the `voxlib` extension by name;
 with `dropin/` on PYTHONPATH that is `dropin/voxlib.py`, which calls `install_import_hook()` below.  The hook waits for
@@ -16,7 +16,7 @@ What is replaced.
     more: the tiles it cuts are VIEWS of the frame-sized tensors `voxlib.ray_voxel_intersection_perspective` returned, so
     the first tile of a frame triggers ONE fused launch over the whole padded frame (`_FrameCache`) and every tile --
     this one included -- gets its window of that result (per-pixel features do not depend on tile boundaries:
-    deterministic sampling, frame-global `sky_avg`; SURVEY.md appendix A "Tiling equivalence").  No redundant rays, one
+    deterministic sampling, frame-global `sky_avg`; DESIGN.md section 1, "Tiling equivalence").  No redundant rays, one
     launch per frame.
 
 Cache validity (the weights may change between calls in ways torch's version counter does not see -- `param.data.copy_()`
@@ -309,7 +309,7 @@ def fused_forward_global(self, net_out, z):
     """Replacement body of Base3DGenerator._forward_global (gancraft_base.py:588-603): RenderCNN + tanh on the tensor
     cores.  When `net_out` is a tile of the frame the fused per-pixel launch produced (the unmodified tile loop of
     inference_givenstyle), the CNN runs ONCE on the whole padded frame and every tile gets its window: the receptive
-    radius is 4 px, the loop crops pad/2 = 15 px from every tile side (SURVEY.md appendix A).  Calls that need gradients
+    radius is 4 px, the loop crops pad/2 = 15 px from every tile side (DESIGN.md section 1).  Calls that need gradients
     through the CNN (gen_update) keep the reference's cuDNN composition."""
     st = _state(self)
     reference = type(self)._sdb200_reference_forward_global

@@ -286,7 +286,7 @@ def pose_stats(voxel_id, depth2, n_bins=680, out=None):
 # diagnostics
 # ------------------------------------------------------------------------------------------------
 def tc_selftest(a, b, bf16=False, variant=0):
-    """C = A @ B^T through the library's tcgen05 path.  a [128,K], b [N,K] fp32 CUDA."""
+    """C = A @ B^T through the library's wgmma path.  a [128,K], b [N,K] fp32 CUDA."""
     _check_input(a, 'a', torch.float32)
     _check_input(b, 'b', torch.float32)
     N, K = b.shape

@@ -336,7 +336,7 @@ class FusedPerPixelRenderer:
         self.base_res, self.log2_T, self.L = base_res, log2_T, L
         self.invalidate()
         self.lut_dev = None
-        self.sky_impl = 'native'     # 'native' = sdb_sky_forward (tcgen05), 'torch' = cuBLAS cross-check
+        self.sky_impl = 'native'     # 'native' = sdb_sky_forward (wgmma), 'torch' = cuBLAS cross-check
         self.early_stop = None       # None = module default EARLY_STOP_T, 0 = off
 
     # Cache keys hold a REFERENCE to the keyed tensor (so its address cannot be recycled for another tensor while the
@@ -574,7 +574,7 @@ class _FusedRenderTrainFn(torch.autograd.Function):
 
 
 class _SkyTrainFn(torch.autograd.Function):
-    """sky [1,H,W,64] = SKYMLP(PE(raydirs)) on the tcgen05 engine, differentiable w.r.t. the weights.
+    """sky [1,H,W,64] = SKYMLP(PE(raydirs)) on the wgmma engine, differentiable w.r.t. the weights.
     b1 is the effective layer-0 bias fc1.bias + fc_z_a(z) (gancraft_base.py:159-160), formed by the caller in torch."""
 
     @staticmethod

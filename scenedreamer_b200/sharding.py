@@ -1,4 +1,4 @@
-"""Multi-GPU sharding of the render path (SURVEY.md section 8e).
+"""Multi-GPU sharding of the render path.
 
 Rays are independent given replicated read-only state (voxel volume, hash table, MLP weights), so
 frames shard across ranks with NO data-path collective; the single collective of the path is one
@@ -38,8 +38,8 @@ def cyclic_bands(H, rank, world_size, band_tiles=2, tile_h=8):
     """Single-frame sharding, balanced without knowing the cost profile: the frame is cut into thin bands of `band_tiles`
     tile rows and band b goes to rank b mod world_size.  (The cost of a row is neither flat nor monotonic -- sky at the top
     is free, near ground at the bottom terminates within a few samples, the horizon in the middle is the expensive part -- so
-    one contiguous band per rank, or a band paired with its mirror, leave some ranks idle: 0.1 vs 3.1 ms of kernel time at 8 GPUs,
-    profiles/r02_scale_n8_strong.json, r02_scale_rayslots_n8_strong.json.)
+    one contiguous band per rank, or a band paired with its mirror, leave some ranks idle.  The band height of 2 tile rows was
+    chosen on an 8-GPU box of the previous GPU generation and is carried over untested on H100.)
     Returns the rank's bands as (y0, y1) in frame order; every rank gets the same NUMBER of slots, trailing ones may be empty."""
     bh = band_tiles * tile_h if world_size > 1 else H          # one GPU: the frame is one band
     n_bands = (H + bh - 1) // bh

@@ -1,4 +1,4 @@
-"""Synthetic scenes and evaluation cameras (SURVEY.md section 8d).
+"""Synthetic scenes and evaluation cameras.
 
 No checkpoint, terrain library or dataset is available offline, so benchmarks and tests render a
 seeded procedural scene.  The voxelisation restates what the reference's PCGVoxelGenerator does

@@ -1,15 +1,15 @@
 """Generate tests/golden/*.npz by running the REFERENCE's own pure-PyTorch code on CPU.
 
-Run in the build container only (needs /root/reference, which does not exist on the GPU box):
+Run where the reference's sources are available (SD_REFERENCE_ROOT):
 
     python tests/golden/make_golden.py
 
-The reference cannot travel, so the vectors are committed as small fixtures together with this
-script (task section 3).  Native-only reference ops (voxlib / gridencoder CUDA extensions) are
+The reference's sources are not part of this repository, so the vectors are committed as small
+fixtures together with this script.  Native-only reference ops (voxlib / gridencoder CUDA extensions) are
 not runnable on CPU; where the reference's Python calls them, this script plugs in
   * the reference's own pure-PyTorch positional_encoding_pt for voxlib.positional_encoding, and
   * the oracle's hash-grid encoder (itself checked against the reference CUDA extension on the
-    GPU box by tests/test_vs_reference_gpu.py)
+    GPU by tests/test_gpu_ops.py)
 so that `_forward_perpix` (imaginaire/generators/scenedreamer.py:313-428) runs unmodified.
 """
 import os
@@ -37,7 +37,7 @@ def _stub(name, **attrs):
 
 
 def install_stubs():
-    # import-time dependencies that are absent offline and never executed on this path (SURVEY 8b)
+    # import-time dependencies that are absent offline and never executed on this path
     _stub('upfirdn2d_cuda')
     _stub('bias_act_cuda')
     _stub('imageio')

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Timings of the ops either side of the fused per-pixel kernel (SURVEY.md 8(b) boundary ops and 8(f) rows), each next to the
+"""Timings of the ops either side of the fused per-pixel kernel, each next to the
 reference's own implementation of the same op on the same GPU / host.  Not the headline metric (bench.py is); this is the
 measurement for rows a1, a6/a7 (stand-alone), f1, f2, f3, f4 and the `voxlib` surface.
 

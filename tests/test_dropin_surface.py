@@ -26,7 +26,7 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(L, name), 'libsdb200.so does not export %s' % name
         assert name in _lib.SIGNATURES, 'scenedreamer_b200/_lib.py has no signature for %s' % name
     assert L.sdb_version() >= 100
-    assert b'sm_100a' in L.sdb_build_info()
+    assert b'sm_90a' in L.sdb_build_info()
     assert b'invalid' in L.sdb_error_string(-1)
     # host-only entry point: camera frame matches the oracle bit for bit
     import oracle
@@ -101,7 +101,7 @@ def test_voxlib_and_gridencoder_module_surface(dropin_path):
         voxlib.positional_encoding(torch.zeros(3, 3), 2, -1, True)
     with pytest.raises(RuntimeError):
         voxlib.sp_trilinear_worldcoord(torch.zeros(4, 2), torch.zeros(2, 2, 2, dtype=torch.int32), torch.zeros(3, 3), False, -1)
-    # import-time stand-ins of the two StyleGAN2 extensions imaginaire.layers hard-imports (SURVEY 8b)
+    # import-time stand-ins of the two StyleGAN2 extensions imaginaire.layers hard-imports
     import bias_act_cuda
     import upfirdn2d_cuda
     with pytest.raises(RuntimeError):

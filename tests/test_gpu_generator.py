@@ -1,5 +1,5 @@
 """The REAL reference Generator (imaginaire.generators.scenedreamer.Generator, unmodified, staged by oracle/build_ref.py)
-rendered twice on the B200 through its own `inference_givenstyle`:
+rendered twice on the GPU through its own `inference_givenstyle`:
 
   arm A  the reference as it ships: its own CUDA extensions (oracle/_ref/*.so), unfused tile loop, cuBLAS fp32 -- in a
          subprocess (`python -m oracle.refgen --backend ref`);
@@ -143,7 +143,7 @@ def test_generator_forward_under_autograd(fused_generator):
     for q in params:
         q.requires_grad_(True)
     if hasattr(gen, 'sky_avg'):
-        del gen.sky_avg                                           # inference leaves it behind (SURVEY appendix A hazard)
+        del gen.sky_avg                                           # inference leaves it behind
     before = gen._sdb200.stats['train_calls']
     try:
         gen.coarse_deterministic_sampling = False

@@ -263,5 +263,5 @@ def test_ray_slots_equal_the_tile_kernel(scene, lut, golden_ops, monkeypatch):
     steps_rq, steps_tile = res[(None, '1')][1], res[(None, '0')][1]
     print('steps of 128 rows: ray slots %d, tiles %d (early termination on); %d / %d with it off'
           % (steps_rq, steps_tile, res[(0.0, '1')][1], res[(0.0, '0')][1]))
-    assert steps_rq > 0 and steps_tile > 0          # (fewer steps only on frame-sized inputs: profiles/r02_ray_stats.log; here the
+    assert steps_rq > 0 and steps_tile > 0          # (fewer steps only on frame-sized inputs, tools/ray_stats.py; here the
                                                     #  per-CTA drain of a 3,000-ray window dominates: 603 vs 576 steps measured)

@@ -1,7 +1,8 @@
 """Per-layer timeline of the fused render kernel (CTA 0, a few steady-state sample steps), from the clock stamps the kernel
 records when a diagnostics buffer is armed (rf_common.cuh SDB_STAMP).  Workload = bench.py's C2 frame.
 
-    PYTHONPATH=. python tools/render_timeline.py [first_step] > profiles/r02_render_timeline.txt
+    SDB_NVCC_EXTRA=-DSDB_TIMELINE python -m scenedreamer_b200.build --force
+    PYTHONPATH=. python tools/render_timeline.py [first_step]
 """
 import ctypes
 import sys
@@ -30,7 +31,6 @@ L.sdb_debug_set_progress_buffer(ctypes.c_void_p(0))
 t = buf[64:64 + 6 * 8 * 8].cpu().numpy().astype(np.int64).reshape(6, 8, 8) & 0xffffffff
 NL = 7
 names = ['fc_1', 'fc_2', 'fc_3', 'fc_4', 'fc_5', 'fc_6', 'out_c']
-mma = [27 * 128, 50 * 128, 50 * 128, 50 * 128, 50 * 128, 50 * 128, 50 * 32]
 
 
 def d(a, b):
@@ -38,29 +38,23 @@ def d(a, b):
 
 
 print('# cycles (SM clock), CTA 0, sample steps %d..%d of its ray slots; per layer:' % (first, first + 5))
-print('#  issue   = issuer: first operand wait of the layer -> last MMA issued      mma_floor = MMAs x 128 (x 32 for N=64) cycles')
-print('#  drain   = last MMA issued -> accumulator complete seen by the epilogue (half 0)')
-print('#  epi     = accumulator complete -> last slab handed over (max of the two halves)')
-print('#  next    = last MMA of this layer issued -> first operand wait of the next layer done (issuer idle)')
-print('%-6s %9s %9s %7s %7s %7s %7s' % ('layer', 'mma_floor', 'issue', 'drain', 'epi', 'next', 'period'))
-tot = np.zeros(5)
-cnt = 0
+print('#  compute = MMA warpgroup: inputs of the layer ready -> its accumulators written')
+print('#  hand    = accumulators written -> seen by the epilogue (half 0)')
+print('#  epi     = accumulators seen -> last slab handed over (max of the two halves)')
+print('#  next    = accumulators written -> inputs of the next layer ready (MMA warpgroup idle)')
+print('%-6s %9s %7s %7s %7s %7s' % ('layer', 'compute', 'hand', 'epi', 'next', 'period'))
 for s in range(1, 5):
     for l in range(NL):
         r = t[s, l]
         nxt = t[s, l + 1][0] if l + 1 < NL else t[s + 1, 0][0]
-        prev0 = t[s, l][0]
-        row = [d(r[1], r[0]), d(r[2], r[1]), max(d(r[3], r[2]), d(r[5], r[4])), d(nxt, r[1]), d(nxt, prev0)]
+        row = [d(r[1], r[0]), d(r[2], r[1]), max(d(r[3], r[2]), d(r[5], r[4])), d(nxt, r[1]), d(nxt, r[0])]
         if s == 2:
-            print('%-6s %9d %9d %7d %7d %7d %7d' % (names[l], mma[l], *row))
-    step = d(t[s + 1, 0][0], t[s, 0][0])
-    tot += np.array([sum(mma), step, 0, 0, 0])
-    cnt += 1
-print('# gather role preparing step n+1, relative to the issuer entering fc_1 of step n (cycles): start (compositing of n-1 seen), slots refilled,')
+            print('%-6s %9d %7d %7d %7d %7d' % (names[l], *row))
+print('# gather role preparing step n+1, relative to the MMA warpgroup entering fc_1 of step n (cycles): start (compositing of n-1 seen), slots refilled,')
 print('#   features gathered (all loads + interpolation done), operand buffer free (colour-layer MMAs of step n retired)')
 for s in range(1, 5):
     g = t[s + 1, 7]
     base = t[s, 0][0]
-    print('gather for step %d: %s   | issuer layer starts of step %d: %s' % (first + s + 1, [d(g[k], base) for k in range(4)], first + s,
+    print('gather for step %d: %s   | MMA layer starts of step %d: %s' % (first + s + 1, [d(g[k], base) for k in range(4)], first + s,
                                                                               [d(t[s, l][0], base) for l in range(NL)]))
-print('step period (issuer, fc_1 to fc_1): %s cycles; MMA floor per step %d' % ([d(t[s + 1, 0][0], t[s, 0][0]) for s in range(0, 5)], sum(mma)))
+print('step period (MMA warpgroup, fc_1 to fc_1): %s cycles' % [d(t[s + 1, 0][0], t[s, 0][0]) for s in range(0, 5)])

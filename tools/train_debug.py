@@ -1,4 +1,4 @@
-"""Stage-by-stage diagnostics of the fused training path on the GPU box (not a test; prints a table).
+"""Stage-by-stage diagnostics of the fused training path on the GPU (not a test; prints a table).
 
 Every stage of sdb_render_rays_train_forward / sdb_render_rays_backward is compared with plain torch fp32 on the
 GPU, using the library's OWN recorded inputs of that stage, so a wrong stage is visible in isolation:
