@@ -23,7 +23,8 @@
 //   * accumulators: a layer's fp32 [128 x 256] result (128 KB) fits neither next to the operand buffers in
 //     shared memory nor in the registers the three roles share, so the MMA warpgroup writes it to a
 //     per-CTA buffer pair in global memory (L2-resident, ping-pong by layer parity) and the epilogue reads
-//     its rows from there; a layer starts when the epilogue has written all of its input;
+//     its rows from there; MMA and epilogue hand a layer over per 64-row block, so the epilogue of one row block
+//     runs while the MMAs of the other do;
 //   * bias, style beta and the label embedding ride in the GEMM: the operand has 16 extra K columns
 //     (one-hot label + constant 1), the weight image carries bias / embedding rows there -- exactly
 //     the reference's fc_m_a(onehot) product -- so the epilogue is LeakyReLU + 16-bit split only;
@@ -240,6 +241,7 @@ mlp_kernel(const Params p)
     constexpr bool ESTOP = MODE == kRender && !TRAIN;
     volatile int *sStop = reinterpret_cast<volatile int *>(smem + SM.stop);
     volatile int *sVote = sStop + 2;
+    int *sVoted = const_cast<int *>(sStop) + 4;  // row blocks that have voted on step s (index s & 1)
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     // the render gradient chain has no dependency between the sample steps of a tile: there every (tile, step) is its own
@@ -261,16 +263,18 @@ mlp_kernel(const Params p)
         for (int i = 0; i < 4; i++) tc05::mbar_init(&bars[B_WFULL + i], 1);
         tc05::mbar_init(&bars[B_FEAT], kGatherThreads);
         tc05::mbar_init(&bars[B_HFREE], 1);
-        for (int i = 0; i < 16; i++) tc05::mbar_init(&bars[B_CHUNK + i], kEpiThreads / 2);
-        tc05::mbar_init(&bars[B_ACC], 1);
-        tc05::mbar_init(&bars[B_OUTRDY], 1);
-        tc05::mbar_init(&bars[B_EPIDONE], kEpiThreads);
-        tc05::mbar_init(&bars[B_EPIDONE + 1], kEpiThreads);
+        for (int rb = 0; rb < 2; rb++) {
+            tc05::mbar_init(&bars[B_OPND + rb], kEpiThreads / 2);
+            tc05::mbar_init(&bars[B_ACC + rb], 1);
+            tc05::mbar_init(&bars[B_OUTRDY + rb], 1);
+            tc05::mbar_init(&bars[B_EPIDONE + rb], kEpiThreads / 2);
+            tc05::mbar_init(&bars[B_EPIDONE + 2 + rb], kEpiThreads / 2);
+        }
         for (int i = 0; i < 2; i++) { tc05::mbar_init(&bars[B_STRDY + i], kRows); tc05::mbar_init(&bars[B_STFREE + i], kEpiThreads); }
         tc05::mbar_init(&bars[B_COMP], kEpiThreads);
         tc05::fence_mbar_init();
     }
-    if (tid < 2) { sStop[tid] = RAYQ ? 0x7fffffff : kMaxS + 1; sVote[tid] = 0; }
+    if (tid < 2) { sStop[tid] = RAYQ ? 0x7fffffff : kMaxS + 1; sVote[tid] = 0; sVoted[tid] = 0; }
     if constexpr (RAYQ) {
         for (int i = tid; i < kRows; i += kThreads) { sCur[i] = make_int2(-1, 0); sDone[i] = 0; sDone[kRows + i] = 0; }
         if (tid < 5) sExh[tid] = 0;
@@ -311,6 +315,21 @@ mlp_kernel(const Params p)
     if (warp < 8) {
         // =========================== EPILOGUE / COMPOSITING WARPS ===========================
         const int row = tid & (kRows - 1), half = tid >> 7;          // column half: 128*half .. +127
+        // 64-row block of this thread (warps 0,1,4,5 / 2,3,6,7): its hand-offs with the MMA warpgroup and its compositing
+        // barrier (named barrier 4 + rb) are per row block, so the two blocks can run up to half a layer apart
+        const int rb = row >> 6;
+        const bool rb_lead = (tid & 191) == 0;                       // thread 0 / 64: one per row block
+        // early-termination vote of step s: a row-block leader calls this once its block's votes are in; the second of the two
+        // blocks gets true and decides for the CTA from the votes of both
+        auto last_vote = [&](int s) {
+            __threadfence_block();
+            const bool last = atomicAdd(&sVoted[s & 1], 1) == 1;
+            if (last) {
+                sVoted[s & 1] = 0;
+                __threadfence_block();
+            }
+            return last;
+        };
         const float *acc_row = p.acc + (size_t)blockIdx.x * 2 * kRows * kHidden + (size_t)row * kHidden;   // accumulator row
         uint32_t n = 0;                 // global step counter
         int loaded_img = -1;
@@ -377,9 +396,9 @@ mlp_kernel(const Params p)
                     if constexpr (BWD)
                         mw = __ldg(reinterpret_cast<const uint4 *>(p.tr.mask + ((step_id * kNumAct + (NACT - 1 - l)) * kRows + row) * 8 + half * 4));
                     if ((tid & 127) == 0) SDB_MARK(half, 1, n, l);
-                    tc05::mbar_wait(&bars[B_ACC], (n * NH + l) & 1);
+                    tc05::mbar_wait(&bars[B_ACC + rb], (n * NH + l) & 1);
                     if ((tid & 127) == 0) SDB_MARK(half, 2, n, l);
-                    if ((tid & 127) == 0) SDB_STAMP(n, l, 2 + 2 * half);
+                    if (rb_lead) SDB_STAMP(n, l, 4 + 2 * rb);
 #pragma unroll 1
                     for (int c0 = 0; c0 < 128; c0 += 32) {
                         // a 32-column chunk in two 16-column halves (16 live accumulator registers instead of 32: the
@@ -428,12 +447,7 @@ mlp_kernel(const Params p)
                                 *reinterpret_cast<uint4 *>(sHhi + off) = hi;
                                 if constexpr (X3) *reinterpret_cast<uint4 *>(sHlo + off) = lo;
                             }
-                            // a 16-column K slab of the next layer's operand is complete (all 128 rows once the four quadrant
-                            // warps of this half have arrived): the MMA issuer may start on it
-                            tc05::fence_proxy_async_smem();
-                            tc05::mbar_arrive(&bars[B_CHUNK + half * 8 + (c0 >> 4) + hh]);
                         }
-                        // the training record is written AFTER the chunk has been handed to the MMA issuer (off the critical path)
                         if constexpr (TRAIN || BWD) {
                             // forward: A_{l+1}[slot][128*half + c0 ..], backward: dZ_{6-l}[slot][...]
                             // (tiled record: a warp's 32 rows of one 8-column chunk are 512 contiguous bytes)
@@ -448,8 +462,12 @@ mlp_kernel(const Params p)
                         }
                         if constexpr (TRAIN) p.tr.mask[((step_id * kNumAct + l) * kRows + row) * 8 + half * 4 + (c0 >> 5)] = mword;
                     }
-                    tc05::mbar_arrive(&bars[B_EPIDONE + (g & 1u)]);        // accumulator buffer (g & 1) is free again
-                    if ((tid & 127) == 0) SDB_STAMP(n, l, 3 + 2 * half);
+                    // the next layer's operand rows of this row block are written (the MMA warpgroup may start on them), and
+                    // these rows of accumulator buffer (g & 1) are free again
+                    tc05::fence_proxy_async_smem();
+                    tc05::mbar_arrive(&bars[B_OPND + rb]);
+                    tc05::mbar_arrive(&bars[B_EPIDONE + (g & 1u) * 2 + rb]);
+                    if (rb_lead) SDB_STAMP(n, l, 5 + 2 * rb);
                     if (MODE == kRender && l == 3) sSig[half * kRows + row] = sig_part;
                     if constexpr (TRAIN) {   // the constant-1 column that turns the weight-gradient GEMM's column 256 into the bias gradient
                         if (half == 0) {
@@ -462,9 +480,9 @@ mlp_kernel(const Params p)
                 // ---- colour layer ----
                 const uint32_t go = n * NL + NH;
                 if ((tid & 127) == 0) SDB_MARK(half, 3, n, NH);
-                tc05::mbar_wait(&bars[B_OUTRDY], n & 1);
+                tc05::mbar_wait(&bars[B_OUTRDY + rb], n & 1);
                 if ((tid & 127) == 0) SDB_MARK(half, 4, n, NH);
-                if ((tid & 127) == 0) SDB_STAMP(n, NH, 2 + 2 * half);
+                if (rb_lead) SDB_STAMP(n, NH, 4 + 2 * rb);
                 if constexpr (SKYBWD) {
                     // last layer of the sky chain: dA1 [128 x 256] -> dZ1 = dA1 * LeakyReLU'(z1) -> bf16 record only
                     const uint4 mw = __ldg(reinterpret_cast<const uint4 *>(p.tr.mask + ((step_id * kNumAct + 0) * kRows + row) * 8 + half * 4));
@@ -482,8 +500,8 @@ mlp_kernel(const Params p)
                                 make_uint4(tc05::pack2<true>(v[8 * q], v[8 * q + 1]), tc05::pack2<true>(v[8 * q + 2], v[8 * q + 3]),
                                            tc05::pack2<true>(v[8 * q + 4], v[8 * q + 5]), tc05::pack2<true>(v[8 * q + 6], v[8 * q + 7]));
                     }
-                    tc05::mbar_arrive(&bars[B_EPIDONE + (go & 1u)]);
-                    if ((tid & 127) == 0) SDB_STAMP(n, NH, 3 + 2 * half);
+                    tc05::mbar_arrive(&bars[B_EPIDONE + (go & 1u) * 2 + rb]);
+                    if (rb_lead) SDB_STAMP(n, NH, 5 + 2 * rb);
                     continue;
                 }
                 float c[32];
@@ -492,8 +510,8 @@ mlp_kernel(const Params p)
                     // d(hash-grid features) [128 rays x 128]: this half owns 64 columns -> fp32 record for the table backward
                     float c2[32];
                     acc_ld<32>(acc_row + (go & 1u) * kRows * kHidden + half * 64 + 32, c2);
-                    tc05::mbar_arrive(&bars[B_EPIDONE + (go & 1u)]);
-                    if ((tid & 127) == 0) SDB_STAMP(n, NH, 3 + 2 * half);
+                    tc05::mbar_arrive(&bars[B_EPIDONE + (go & 1u) * 2 + rb]);
+                    if (rb_lead) SDB_STAMP(n, NH, 5 + 2 * rb);
                     float *dst = p.tr.dx0 + slot * kFeat + half * 64;
 #pragma unroll
                     for (int q = 0; q < 4; q++) st_global_v8f(dst + 8 * q, &c[8 * q]);
@@ -501,14 +519,14 @@ mlp_kernel(const Params p)
                     for (int q = 0; q < 4; q++) st_global_v8f(dst + 32 + 8 * q, &c2[8 * q]);
                     continue;
                 }
-                tc05::mbar_arrive(&bars[B_EPIDONE + (go & 1u)]);
-                if ((tid & 127) == 0) SDB_STAMP(n, NH, 3 + 2 * half);
+                tc05::mbar_arrive(&bars[B_EPIDONE + (go & 1u) * 2 + rb]);
+                if (rb_lead) SDB_STAMP(n, NH, 5 + 2 * rb);
                 if constexpr (SKY) {
 #pragma unroll
                     for (int j = 0; j < 32; j++) outc[j] = c[j];
                 } else if constexpr (RAYQ) {
                     // ---- compositing of ray slots (a10/a11): every row is its own ray at its own sample step ----
-                    asm volatile("bar.sync 1, 256;" ::: "memory");
+                    tc05::named_sync(4 + rb, 128);                          // sSig of both column halves of these rows
                     const float sigma = (sSig[row] + sSig[kRows + row]) + sF[kFBsig];
                     const uint4 info = sInfo[(s & 3) * kRows + row];            // published by the gather role for this step
                     const int rq = (int)info.z;
@@ -575,8 +593,8 @@ mlp_kernel(const Params p)
                         const bool idle = !act || fin;
                         const bool wall = __all_sync(0xffffffffu, idle);
                         if (lane == 0 && !wall) sVote[s & 1] = 1;
-                        asm volatile("bar.sync 1, 256;" ::: "memory");
-                        if (tid == 0) {
+                        tc05::named_sync(4 + rb, 128);
+                        if (rb_lead && last_vote(s)) {
                             if (sVote[s & 1] == 0 && sExh[s & 3] != 0 && sStop[0] > s + 2) sStop[0] = s + 2;
                             sVote[s & 1] = 0;
                         }
@@ -584,7 +602,7 @@ mlp_kernel(const Params p)
                     tc05::mbar_arrive(&bars[B_COMP]);                      // compositing of step s is complete (done flags visible)
                 } else {
                     // ---- compositing (a10/a11) ----
-                    asm volatile("bar.sync 1, 256;" ::: "memory");
+                    tc05::named_sync(4 + rb, 128);                          // sSig of both column halves of these rows
                     const float sigma = (sSig[row] + sSig[kRows + row]) + sF[kFBsig];
                     const float e = __fmul_rn(fmaxf(sigma, 0.0f), __fmul_rn(sm.nd, p.dists_scale));   // mc_utils.py:155
                     const float a = 1.0f - expf(-e);
@@ -617,8 +635,8 @@ mlp_kernel(const Params p)
                         const bool done = !live || expf(-Eexcl) < p.early_T;
                         const bool wall = __all_sync(0xffffffffu, done);
                         if (lane == 0 && !wall) sVote[s & 1] = 1;
-                        asm volatile("bar.sync 1, 256;" ::: "memory");
-                        if (tid == 0) {
+                        tc05::named_sync(4 + rb, 128);
+                        if (rb_lead && last_vote(s)) {
                             if (sVote[s & 1] == 0 && sStop[buf] > S) sStop[buf] = s + 2;
                             sVote[s & 1] = 0;
                         }
@@ -698,124 +716,129 @@ mlp_kernel(const Params p)
     } else if (warp < kGatherWarp0) {
       asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegsCtl));
       // =========================== MMA WARPGROUP ===========================
-      // Layer l of a sample step: D[128 x N] = H[128 x K] * W_l^T, computed in 64-row x 32-column blocks (the sum over K in
-      // registers), each written once to this CTA's fp32 accumulator buffer (g & 1) in global memory, where the epilogue reads
-      // its rows.  Weights go through a 4-slot ring of 16 KB stages = up to 8 k16 slabs of one 32-column block; thread 0
-      // issues the bulk copies up to 3 stages ahead of the MMAs.  Named barrier 3 is this warpgroup's (1: epilogue, 2: gather).
+      // Layer l of a sample step: D[128 x N] = H[128 x K] * W_l^T, one 64-row block rb after the other, each in 32-column
+      // blocks (the sum over K in registers) written once to this CTA's fp32 accumulator buffer (g & 1) in global memory, where
+      // the epilogue reads its rows.  A row block is handed over as soon as it is written, so the epilogue of one row block runs
+      // while the MMAs of the other do.  Weights go through a 4-slot ring of 16 KB stages = up to 8 k16 slabs of one 32-column
+      // block, one bulk copy each (wpack_off); thread 0 keeps the ring full, the weights are streamed once per row block.
+      // Named barrier 3 is this warpgroup's (1, 4, 5: epilogue, 2: gather).
+      //
+      // Numerics: every stage starts a fresh tensor-core sum that is added to the block's running sum in fp32 with round-to-
+      // nearest, in stage order: the tensor core's own accumulation does not round to nearest, and over a whole x3 layer (up to
+      // 51 chained MMAs) that moved the full-frame depth outside its parity bound.  Two accumulator sets alternate, so that the
+      // add and the ring-slot release of one stage overlap the MMAs of the next.
       const int t = tid - kMmaWarp0 * 32;
       constexpr uint32_t kSlot = 16384, kSlabB = 1024 * PARTS;       // ring slot; one k16 slab of a 32-column block
-      uint32_t n = 0, q0 = 0;                                        // q0: ring stages of all earlier steps
-      auto layer_stages = [&](int l) { return 2 * (layerN<MODE>(l) / 32) * ((layerK<MODE>(l) / 16 + 7) / 8); };
+      uint32_t n = 0, q = 0, qr = 0;                                 // ring stages issued to the tensor cores / retired
       for (int it = 0;; it++) {
           const int work = fetch_work(it);
           if (work < 0) break;
           const int tile = RAYQ ? 0 : (ONE_STEP ? work : p.tile_list[work / wmult]);
           const uint8_t *pack = p.pack + (long long)tile_coord(p, tile).img * p.pack_stride;
-          int n_st = 0;
-          for (int l = 0; l < NL; l++) n_st += layer_stages(l);
-          // stage k of a step -> (layer, 32-column block, first slab, slabs); stages go (layer, row block, column block, slabs)
-          auto issue = [&](int k) {
-              int l = 0;
-              while (k >= layer_stages(l)) { k -= layer_stages(l); l++; }
-              const int N = layerN<MODE>(l), nK = layerK<MODE>(l) / 16, nsg = (nK + 7) / 8;
-              const int blk = k / nsg, sg = k % nsg, cc = blk % (N / 32);
-              const int kk0 = sg * 8;
-              return make_int4(l, cc, kk0, min(8, nK - kk0));
-          };
           for (int s = 0; s < SL; s++, n++) {
               if (ESTOP && s >= 2 && s >= sStop[it & 1]) break;
-              int k = 0, k_issued = 0;
-              auto produce = [&](int upto) {           // thread 0: stages k_issued .. upto - 1 of this step
-                  for (; k_issued < upto && k_issued < n_st; k_issued++) {
-                      const int4 d = issue(k_issued);
-                      const int N = layerN<MODE>(d.x);
-                      const uint32_t q = q0 + (uint32_t)k_issued, slot = q & 3u;
-                      const uint8_t *w = pack + layerOff<MODE>(d.x, PARTS);
-                      const uint32_t slabB = (uint32_t)N * 32u * PARTS;
-                      tc05::mbar_arrive_expect_tx(&bars[B_WFULL + slot], (uint32_t)d.w * kSlabB);
-                      for (int i = 0; i < d.w; i++)
-#pragma unroll
-                          for (int part = 0; part < PARTS; part++)
-#pragma unroll
-                              for (int kc = 0; kc < 2; kc++)
-                                  tc05::bulk_g2s(sRing + slot * kSlot + i * kSlabB + part * 1024 + kc * 512,
-                                                 w + (size_t)(d.z + i) * slabB + part * N * 32 + kc * N * 16 + d.y * 512, 512,
-                                                 &bars[B_WFULL + slot]);
+              // weight loads (thread 0): the stages of a step are, per layer, (row block, 32-column block, slab group); the next
+              // one to load is stage pj of layer pl, ring index pq
+              int pl = 0, pj = 0;
+              uint32_t pq = q;
+              auto produce = [&](uint32_t upto) {
+                  for (; pq < upto && pl < NL; pq++) {
+                      const int nK = layerK<MODE>(pl) / 16, nsg = (nK + 7) / 8, per_rb = layerN<MODE>(pl) / 32 * nsg;
+                      const int j = pj < per_rb ? pj : pj - per_rb, cc = j / nsg, kk0 = (j - cc * nsg) * 8;
+                      const uint32_t bytes = (uint32_t)min(8, nK - kk0) * kSlabB, slot = pq & 3u;
+                      tc05::mbar_arrive_expect_tx(&bars[B_WFULL + slot], bytes);
+                      tc05::bulk_g2s(sRing + slot * kSlot, pack + layerOff<MODE>(pl, PARTS) + wpack_off(nK, PARTS, cc * 32, kk0 * 16, 0),
+                                     bytes, &bars[B_WFULL + slot]);
+                      if (++pj == 2 * per_rb) { pj = 0; pl++; }
                   }
               };
-              if (t == 0) produce(3);
+              if (t == 0) produce(q + 4);
 #pragma unroll 1
               for (int l = 0; l < NL; l++) {
                   const uint32_t g = n * NL + l, buf = g & 1u;
-                  if (t == 0) SDB_MARK(2, 1, n, l);
-                  // accumulator buffer `buf` was last read by the epilogue of global layer g - 2
-                  if (g >= 2) tc05::mbar_wait(&bars[B_EPIDONE + buf], ((g >> 1) - 1) & 1);
-                  if (l == 0) {
-                      tc05::mbar_wait(&bars[B_FEAT], n & 1);
-                  } else {
-                      const uint32_t cpar = (n * NH + l - 1) & 1;      // operand of this layer from the previous epilogue
-                      for (int c = 0; c < 16; c++) tc05::mbar_wait(&bars[B_CHUNK + c], cpar);
-                  }
-                  if (t == 0) SDB_MARK(2, 2, n, l);
-                  if (t == 0) SDB_STAMP(n, l, 0);
-                  const int N = layerN<MODE>(l), nK = layerK<MODE>(l) / 16, nsg = (nK + 7) / 8;
-                  float *dst = p.acc + ((size_t)blockIdx.x * 2 + buf) * kRows * kHidden;
+                  const int N = layerN<MODE>(l), nK = layerK<MODE>(l) / 16, nsg = (nK + 7) / 8, nst = N / 32 * nsg;
 #pragma unroll 1
                   for (int rb = 0; rb < 2; rb++) {
-#pragma unroll 1
-                      for (int cc = 0; cc < N / 32; cc++) {
-                          float d[16], sum[16];
-#pragma unroll 1
-                          for (int sg = 0; sg < nsg; sg++, k++) {
-                              if (t == 0) produce(k + 4);
-                              const uint32_t q = q0 + (uint32_t)k, slot = q & 3u;
-                              tc05::mbar_wait(&bars[B_WFULL + slot], (q >> 2) & 1u);
-                              const uint32_t sb = tc05::smem_u32(sRing + slot * kSlot);
-                              const int kk0 = sg * 8, ns = min(8, nK - kk0);
-                              tc05::wgmma_fence();
-#pragma unroll 1
-                              for (int i = 0; i < ns; i++) {
-                                  const uint32_t aoff = (uint32_t)(kk0 + i) * 2 * kLboA + rb * 1024;
-                                  const uint64_t ah = tc05::make_smem_desc(tc05::smem_u32(sHhi) + aoff, kLboA, kSbo);
-                                  const uint64_t bh = tc05::make_smem_desc(sb + i * kSlabB, 512, kSbo);
-                                  tc05::wgmma_m64n32k16<BF16, 0, 0>(d, ah, bh, i > 0 ? 1u : 0u);
-                                  if constexpr (X3) {
-                                      const uint64_t al = tc05::make_smem_desc(tc05::smem_u32(sHlo) + aoff, kLboA, kSbo);
-                                      tc05::wgmma_m64n32k16<BF16, 0, 0>(d, al, bh, 1u);
-                                      tc05::wgmma_m64n32k16<BF16, 0, 0>(d, ah, bh + (1024 >> 4), 1u);
-                                  }
-                              }
-                              tc05::wgmma_commit();
-                              tc05::wgmma_wait<0>();
-                              tc05::wgmma_fence_acc(d);
-                              tc05::named_sync(3, 128);           // every warp is done with the slot: it may be refilled
-                              // Every stage (<= 8 k16 slabs) starts a fresh tensor-core sum, added to the running sum in fp32
-                              // with round-to-nearest: the tensor core's own accumulation does not round to nearest, and over a
-                              // whole x3 layer (up to 51 chained MMAs) that moved the full-frame depth outside its parity bound.
-#pragma unroll
-                              for (int i = 0; i < 16; i++) sum[i] = sg == 0 ? d[i] : __fadd_rn(sum[i], d[i]);
-                          }
-#ifndef SDB_AB_NO_ACC
-#pragma unroll
-                          for (int i = 0; i < 16; i += 2)
-                              *reinterpret_cast<float2 *>(dst + (size_t)(rb * 64 + tc05::frag_row(t, i)) * kHidden + cc * 32 +
-                                                          tc05::frag_col(t, i)) = make_float2(sum[i], sum[i + 1]);
-#endif
-                      }
-                  }
-                  __threadfence_block();
-                  tc05::named_sync(3, 128);
-                  if (t == 0) SDB_STAMP(n, l, 1);
-                  if (t == 0) {
-                      if (l == NL - 1) {
-                          tc05::mbar_arrive(&bars[B_OUTRDY]);
-                          tc05::mbar_arrive(&bars[B_HFREE]);
+                      if (t == 0) SDB_MARK(2, 1, n, l);
+                      // these rows of accumulator buffer `buf` were last read by the epilogue of global layer g - 2
+                      if (g >= 2) tc05::mbar_wait(&bars[B_EPIDONE + buf * 2 + rb], ((g >> 1) - 1) & 1);
+                      if (l == 0) {
+                          if (rb == 0) tc05::mbar_wait(&bars[B_FEAT], n & 1);
                       } else {
-                          tc05::mbar_arrive(&bars[B_ACC]);
+                          tc05::mbar_wait(&bars[B_OPND + rb], (n * NH + l - 1) & 1);   // operand rows from the previous epilogue
+                      }
+                      if (t == 0) SDB_MARK(2, 2, n, l);
+                      if (t == 0) SDB_STAMP(n, l, 2 * rb);
+                      float *dst = p.acc + (((size_t)blockIdx.x * 2 + buf) * kRows + rb * 64) * kHidden;
+                      float da[16], db[16], sum[16];
+                      // stage j of this row block (32-column block j / nsg, slab group j % nsg): issue its MMAs into d
+                      auto mma = [&](float (&d)[16], int j) {
+                          const uint32_t slot = q & 3u;
+                          tc05::mbar_wait(&bars[B_WFULL + slot], (q >> 2) & 1u);
+                          const uint32_t sb = tc05::smem_u32(sRing + slot * kSlot);
+                          const int kk0 = (j % nsg) * 8, ns = min(8, nK - kk0);
+                          tc05::wgmma_fence();
+#pragma unroll
+                          for (int i = 0; i < 8; i++) {
+                              if (i >= ns) break;
+                              const uint32_t aoff = (uint32_t)(kk0 + i) * 2 * kLboA + rb * 1024;
+                              const uint64_t ah = tc05::make_smem_desc(tc05::smem_u32(sHhi) + aoff, kLboA, kSbo);
+                              const uint64_t bh = tc05::make_smem_desc(sb + i * kSlabB, 512, kSbo);
+                              tc05::wgmma_m64n32k16<BF16, 0, 0>(d, ah, bh, i > 0 ? 1u : 0u);
+                              if constexpr (X3) {
+                                  const uint64_t al = tc05::make_smem_desc(tc05::smem_u32(sHlo) + aoff, kLboA, kSbo);
+                                  tc05::wgmma_m64n32k16<BF16, 0, 0>(d, al, bh, 1u);
+                                  tc05::wgmma_m64n32k16<BF16, 0, 0>(d, ah, bh + (1024 >> 4), 1u);
+                              }
+                          }
+                          tc05::wgmma_commit();
+                          q++;
+                      };
+                      // the MMAs of stage j (in d) are complete: refill its ring slot, add its sum, store a finished block
+                      auto retire = [&](float (&d)[16], int j) {
+                          tc05::wgmma_fence_acc(d);
+                          tc05::named_sync(3, 128);           // every warp is done with the slot
+                          if (t == 0) produce(qr + 5);
+                          qr++;
+                          const int cc = j / nsg, sg = j - cc * nsg;
+#pragma unroll
+                          for (int i = 0; i < 16; i++) sum[i] = sg == 0 ? d[i] : __fadd_rn(sum[i], d[i]);
+#ifndef SDB_AB_NO_ACC
+                          if (sg == nsg - 1) {
+#pragma unroll
+                              for (int i = 0; i < 16; i += 2)
+                                  *reinterpret_cast<float2 *>(dst + (size_t)tc05::frag_row(t, i) * kHidden + cc * 32 + tc05::frag_col(t, i)) =
+                                      make_float2(sum[i], sum[i + 1]);
+                          }
+#endif
+                      };
+                      static_assert(kHidden % 64 == 0 && kOutC % 64 == 0 && kFeat % 64 == 0, "stages go in pairs: every N is a multiple of 64");
+#pragma unroll 1
+                      for (int j = 0; j < nst; j += 2) {
+                          mma(da, j);
+                          if (j > 0) {
+                              tc05::wgmma_wait<1>();
+                              retire(db, j - 1);
+                          }
+                          mma(db, j + 1);
+                          tc05::wgmma_wait<1>();
+                          retire(da, j);
+                      }
+                      tc05::wgmma_wait<0>();
+                      retire(db, nst - 1);
+                      __threadfence_block();
+                      tc05::named_sync(3, 128);
+                      if (t == 0) SDB_STAMP(n, l, 2 * rb + 1);
+                      if (t == 0) {
+                          if (l == NL - 1) {
+                              tc05::mbar_arrive(&bars[B_OUTRDY + rb]);
+                              if (rb == 1) tc05::mbar_arrive(&bars[B_HFREE]);
+                          } else {
+                              tc05::mbar_arrive(&bars[B_ACC + rb]);
+                          }
                       }
                   }
               }
-              q0 += (uint32_t)n_st;
           }
       }
     } else {
@@ -1368,7 +1391,7 @@ pack_kernel(const float *w0, const float *b0, const float *emb, int n_labels, co
         long long r = t;
         int l = 0;
         while (r >= (long long)layerK<MODE>(l) * layerN<MODE>(l)) { r -= (long long)layerK<MODE>(l) * layerN<MODE>(l); l++; }
-        const int K = layerK<MODE>(l), N = layerN<MODE>(l);
+        const int K = layerK<MODE>(l);
         const int nn = (int)(r / K), k = (int)(r % K);
         float v = 0.0f;
         if (l == 0) {
@@ -1387,21 +1410,20 @@ pack_kernel(const float *w0, const float *b0, const float *emb, int n_labels, co
             if (k < kHidden) v = wh[((long long)(l - 1) * kHidden + nn) * kHidden + k];
             else if (k == kHidden) v = bh[(long long)(l - 1) * kHidden + nn];
         }
-        const int kk = k >> 4, k16 = k & 15;
-        const long long slab_off = (long long)(k16 >> 3) * N * 16 + (nn >> 3) * 128 + (nn & 7) * 16 + (k16 & 7) * 2;
-        uint8_t *base = pack + layerOff<MODE>(l, PARTS) + (long long)kk * N * 32 * PARTS;
+        uint8_t *base = pack + layerOff<MODE>(l, PARTS);
+        const int nK = K / 16;
         if constexpr (PREC == 1) {
             const __nv_bfloat16 hi = __float2bfloat16_rn(v);
             const __nv_bfloat16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-            *reinterpret_cast<__nv_bfloat16 *>(base + slab_off) = hi;
-            *reinterpret_cast<__nv_bfloat16 *>(base + (long long)N * 32 + slab_off) = lo;
+            *reinterpret_cast<__nv_bfloat16 *>(base + wpack_off(nK, PARTS, nn, k, 0)) = hi;
+            *reinterpret_cast<__nv_bfloat16 *>(base + wpack_off(nK, PARTS, nn, k, 1)) = lo;
         } else if constexpr (PREC == 2) {
             const __half hi = __float2half_rn(v);
             const __half lo = __float2half_rn(v - __half2float(hi));
-            *reinterpret_cast<__half *>(base + slab_off) = hi;
-            *reinterpret_cast<__half *>(base + (long long)N * 32 + slab_off) = lo;
+            *reinterpret_cast<__half *>(base + wpack_off(nK, PARTS, nn, k, 0)) = hi;
+            *reinterpret_cast<__half *>(base + wpack_off(nK, PARTS, nn, k, 1)) = lo;
         } else {
-            *reinterpret_cast<__half *>(base + slab_off) = __float2half_rn(v);
+            *reinterpret_cast<__half *>(base + wpack_off(nK, PARTS, nn, k, 0)) = __float2half_rn(v);
         }
         return;
     }
@@ -1499,19 +1521,17 @@ pack_bwd_kernel(const float *w1, const float *wh, const float *wsig, const float
         long long r = t;
         int l = 0;
         while (r >= (long long)layerK<MODE>(l) * layerN<MODE>(l)) { r -= (long long)layerK<MODE>(l) * layerN<MODE>(l); l++; }
-        const int K = layerK<MODE>(l), N = layerN<MODE>(l);
+        const int K = layerK<MODE>(l);
         const int nn = (int)(r / K), k = (int)(r % K);
         float v;
         if (l == 0) v = wout[(long long)k * kHidden + nn];
         else if (MODE == kBwd && l == NL - 1) v = w1[(long long)k * kFeat + nn];
         else v = wh[((long long)((MODE == kBwd ? 5 : 4) - l) * kHidden + k) * kHidden + nn];
-        const int kk = k >> 4, k16 = k & 15;
-        const long long slab_off = (long long)(k16 >> 3) * N * 16 + (nn >> 3) * 128 + (nn & 7) * 16 + (k16 & 7) * 2;
-        uint8_t *base = pack + layerOff<MODE>(l, PARTS) + (long long)kk * N * 32 * PARTS;
+        uint8_t *base = pack + layerOff<MODE>(l, PARTS);
         const __nv_bfloat16 hi = __float2bfloat16_rn(v);
         const __nv_bfloat16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-        *reinterpret_cast<__nv_bfloat16 *>(base + slab_off) = hi;
-        *reinterpret_cast<__nv_bfloat16 *>(base + (long long)N * 32 + slab_off) = lo;
+        *reinterpret_cast<__nv_bfloat16 *>(base + wpack_off(K / 16, PARTS, nn, k, 0)) = hi;
+        *reinterpret_cast<__nv_bfloat16 *>(base + wpack_off(K / 16, PARTS, nn, k, 1)) = lo;
         return;
     }
     if (!Net<MODE>::TAIL) return;

@@ -1,5 +1,5 @@
 // Shared definitions of the fused render engine (render_fused.cu) and the training-side kernels
-// (render_train.cu): network shapes, the static weight-ring schedule, the shared-memory map, kernel
+// (render_train.cu): network shapes, the weight-pack layout, the shared-memory map, kernel
 // parameters, ray sampling and hash-grid corner math.  Internal to libsdb200 (not part of the ABI).
 #pragma once
 #include <math.h>
@@ -21,8 +21,9 @@ constexpr int kMmaWarp0 = 8, kGatherWarp0 = 12;
 constexpr int kThreads = kEpiThreads + 128 + kGatherThreads;   // 640
 // setmaxnreg can only redistribute the registers the CTA was LAUNCHED with (640 threads x 96 = 61,440; the
 // allocator is a per-CTA pool -- USETMAXREG.TRY_ALLOC.CTAPOOL spins forever otherwise):
-//   8 epilogue warps x 96 + 4 control warps x 48 + 8 gather warps x 120 = 61,440
-constexpr int kRegsLaunch = 96, kRegsCtl = 48, kRegsGather = 120;
+//   8 epilogue warps x 96 + 4 control warps x 80 + 8 gather warps x 104 = 61,440
+// (the MMA warpgroup holds two 16-register accumulator sets and the running sum: 48 would spill inside its stage loop)
+constexpr int kRegsLaunch = 96, kRegsCtl = 80, kRegsGather = 104;
 static_assert(8 * 32 * kRegsLaunch + 4 * 32 * kRegsCtl + 8 * 32 * kRegsGather <= kThreads * kRegsLaunch,
               "setmaxnreg budget exceeds the CTA's launch-time register allocation");
 constexpr int kRingBytes = 65536;
@@ -63,46 +64,14 @@ constexpr int kFWsig = 0, kFBsig = 256, kFTotal = 264;
 template <int MODE> __host__ __device__ constexpr int64_t packBytes(int parts) {
     return layerOff<MODE>(Net<MODE>::NL, parts) + (Net<MODE>::TAIL ? (int64_t)kFTotal * 4 : 0);
 }
-// Weight-ring schedule.  A ring stage holds KS consecutive k16 slabs (KS = 1 for the x3 modes, 2 for the
-// single-pass mode so that a stage is 16 KB either way).  Layers fed by hidden activations consume the K
-// extension first (no dependency; forward networks only), then the 32-column chunks in the order the two
-// epilogue halves produce them.  Loader and MMA issuer walk the same list.
-template <int KS, int MODE> __host__ __device__ constexpr int num_stages(int l) {
-    return l == 0 ? (Net<MODE>::K0 / 16 + KS - 1) / KS : (Net<MODE>::EXT ? 1 : 0) + 16 / KS;   // [extension +] 8 chunks x (2 / KS)
+// Byte offset of weight element (output n, input k), 16-bit part `part` (hi / lo), inside one layer of the pack, for a layer
+// of nK k16 slabs and `parts` parts.  The layer is stored in the order the MMA warpgroup streams it:
+//   [32-column block n/32][k16 slab k/16][part][k-chunk (k/8)%2][32 outputs][8 k]
+// so one k16 slab of a 32-column block is a 1 KB-per-part wgmma B operand (K-major, no swizzle, LBO 512), and a ring stage
+// (up to 8 consecutive slabs of one block) is ONE contiguous range that a single bulk copy fetches.
+__host__ __device__ constexpr int64_t wpack_off(int nK, int parts, int n, int k, int part) {
+    return ((((int64_t)(n >> 5) * nK + (k >> 4)) * parts + part) * 2 + ((k >> 3) & 1)) * 512 + (n & 31) * 16 + (k & 7) * 2;
 }
-// The epilogue hands the next layer's operand over in 16-column pieces = one k16 slab each: slabs 0..7 come from the
-// epilogue half that owns columns 0..127, slabs 8..15 from the other half, both halves advance together.  Consumption
-// order: KS = 1 (x3 modes, one slab per ring stage): 0,8,1,9,...,7,15; KS = 2 (single-pass mode, two slabs per stage):
-// (0,1),(8,9),(2,3),(10,11),...
-template <int KS> __host__ __device__ constexpr int hidden_stage_slab(int i) {
-    return KS == 1 ? (i >> 1) + (i & 1) * 8 : ((i >> 1) * 2 + (i & 1) * 8);
-}
-template <int KS, int MODE> __host__ __device__ constexpr int stage_kk(int l, int j) {
-    if (l == 0) return j * KS;
-    if (Net<MODE>::EXT && j == 0) return 16;
-    return hidden_stage_slab<KS>(j - (Net<MODE>::EXT ? 1 : 0));
-}
-template <int KS, int MODE> __host__ __device__ constexpr int stage_cnt(int l, int j) {
-    if (l == 0) { const int nk = Net<MODE>::K0 / 16; return (j * KS + KS <= nk) ? KS : nk - j * KS; }
-    return (Net<MODE>::EXT && j == 0) ? 1 : KS;
-}
-// slab barrier to wait on before stage j of a hidden-fed layer (-1: none): the LAST slab of the stage (a half's threads
-// arrive on its slab barriers in order, so that one implies the earlier ones)
-template <int KS, int MODE> __host__ __device__ constexpr int stage_chunk_wait(int l, int j) {
-    if (l == 0 || (Net<MODE>::EXT && j == 0)) return -1;
-    return hidden_stage_slab<KS>(j - (Net<MODE>::EXT ? 1 : 0)) + KS - 1;
-}
-
-// Static schedule: the number of ring stages per sample step is padded to a multiple of the ring depth (4),
-// so the ring slot of every stage is a compile-time constant and its mbarrier parity depends only on the
-// step parity -- the issue loops become straight-line code with immediate addresses.
-template <int KS, int MODE> __host__ __device__ constexpr int stage_index(int l, int j) {
-    int i = j;
-    for (int k = 0; k < l; k++) i += num_stages<KS, MODE>(k);
-    return i;
-}
-template <int KS, int MODE> __host__ __device__ constexpr int stages_per_step() { return stage_index<KS, MODE>(Net<MODE>::NL, 0); }
-template <int KS, int MODE> __host__ __device__ constexpr int stages_per_step_padded() { return (stages_per_step<KS, MODE>() + 3) / 4 * 4; }
 
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
@@ -126,7 +95,7 @@ __host__ __device__ constexpr Smem smem_map(bool x3) {
     m.sig = o; o += 2 * kRows * 4;
     m.state = o; o += 2 * (2 * kMaxM + 6) * kRows * 4;
     m.bars = o; o += 40 * 8;
-    m.stop = o; o += 16;                         // early termination: int stop_step[2] (per tile buffer), int vote[2]
+    m.stop = o; o += 32;                         // early termination: int stop_step[2] (per tile buffer), int vote[2], int voted[2]
     m.sched = o; o += 32;                        // dynamic tile scheduler: int work[4] (ring), int published
     m.total = o;
     return m;
@@ -140,9 +109,10 @@ constexpr int kStLab = 2 * kMaxM + 4;        // 1 (uint32: 4 bits per slot)
 constexpr int kStFlags = 2 * kMaxM + 5;      // 1 (uint32: bit0 live, bit1 sky_mask, bit2 valid)
 constexpr int kStFloats = 2 * kMaxM + 6;
 
-// barrier indices
-enum { B_WFULL = 0, B_WEMPTY = 4, B_FEAT = 8, B_HFREE, B_CHUNK, B_ACC = B_CHUNK + 16, B_OUTRDY, B_EPIDONE,
-       B_STRDY = B_EPIDONE + 2, B_STFREE = B_STRDY + 2, B_COMP = B_STFREE + 2, B_COUNT = B_COMP + 1 };
+// barrier indices.  The MMA warpgroup and the epilogue hand a layer over per 64-row block rb (B_OPND, B_ACC, B_OUTRDY: + rb;
+// B_EPIDONE: + accumulator buffer * 2 + rb), so that one row block's epilogue runs while the other's MMAs do.
+enum { B_WFULL = 0, B_FEAT = 4, B_HFREE, B_OPND, B_ACC = B_OPND + 2, B_OUTRDY = B_ACC + 2, B_EPIDONE = B_OUTRDY + 2,
+       B_STRDY = B_EPIDONE + 4, B_STFREE = B_STRDY + 2, B_COMP = B_STFREE + 2, B_COUNT = B_COMP + 1 };
 constexpr int kBarSlots = 40;
 static_assert(B_COUNT <= kBarSlots, "barrier table");
 
@@ -244,8 +214,9 @@ __device__ __forceinline__ void acc_ld(const float *src, float (&v)[NV]) {
 
 // timeline of CTA 0 (diagnostics, tools/render_timeline.py; library built with SDB_NVCC_EXTRA=-DSDB_TIMELINE): with debug[60] == kTraceMagic, sample steps
 // debug[61] .. debug[61]+kTraceSteps-1 of the CTA record clock() stamps, debug[64 + ((n - first) * 8 + layer) * 8 + slot]:
-//   slot 0 MMA warpgroup: the layer's inputs are ready (buffer free, operand written)   1 MMA warpgroup: the layer's accumulators are written
-//   slot 2/4 epilogue half 0/1: accumulator of the layer complete          3/5 epilogue half 0/1: last slab handed over
+//   slot 2 rb    MMA warpgroup, row block rb: the inputs are ready (buffer free, operand rows written)
+//   slot 2 rb + 1  MMA warpgroup, row block rb: the accumulators are written
+//   slot 4 + 2 rb  epilogue of row block rb: accumulators seen        slot 5 + 2 rb: the next layer's operand rows handed over
 //   layer row 7 = the gather role preparing step n: 0 compositing of step n-2 seen, 1 slots refilled, 2 features gathered, 3 operand buffer free
 constexpr int32_t kTraceMagic = 0x7131;
 constexpr int kTraceSteps = 6;

@@ -37,19 +37,21 @@ def d(a, b):
     return int((a - b) & 0xffffffff) if a and b else -1
 
 
-print('# cycles (SM clock), CTA 0, sample steps %d..%d of its ray slots; per layer:' % (first, first + 5))
-print('#  compute = MMA warpgroup: inputs of the layer ready -> its accumulators written')
-print('#  hand    = accumulators written -> seen by the epilogue (half 0)')
-print('#  epi     = accumulators seen -> last slab handed over (max of the two halves)')
-print('#  next    = accumulators written -> inputs of the next layer ready (MMA warpgroup idle)')
-print('%-6s %9s %7s %7s %7s %7s' % ('layer', 'compute', 'hand', 'epi', 'next', 'period'))
+print('# cycles (SM clock), CTA 0, sample steps %d..%d of its ray slots; per layer and 64-row block rb (0, 1):' % (first, first + 5))
+print('#  mma     = MMA warpgroup: inputs of the row block ready -> its accumulators written')
+print('#  hand    = accumulators written -> seen by the epilogue of that row block')
+print('#  epi     = accumulators seen -> the next layer\'s operand rows handed over')
+print('#  epi0-mma1 = end of row block 0\'s epilogue minus end of row block 1\'s MMAs (<= 0: hidden behind them)')
+print('#  period  = MMA warpgroup: inputs of row block 0 ready -> same for the next layer')
+print('%-6s %7s %7s %7s %7s %7s %7s %9s %7s' % ('layer', 'mma0', 'mma1', 'hand0', 'hand1', 'epi0', 'epi1', 'epi0-mma1', 'period'))
 for s in range(1, 5):
     for l in range(NL):
         r = t[s, l]
         nxt = t[s, l + 1][0] if l + 1 < NL else t[s + 1, 0][0]
-        row = [d(r[1], r[0]), d(r[2], r[1]), max(d(r[3], r[2]), d(r[5], r[4])), d(nxt, r[1]), d(nxt, r[0])]
+        row = [d(r[1], r[0]), d(r[3], r[2]), d(r[4], r[1]), d(r[6], r[3]), d(r[5], r[4]), d(r[7], r[6]),
+               (int((r[5] - r[3] + 2**31) & 0xffffffff) - 2**31) if r[5] and r[3] else -1, d(nxt, r[0])]
         if s == 2:
-            print('%-6s %9d %7d %7d %7d %7d' % (names[l], *row))
+            print('%-6s %7d %7d %7d %7d %7d %7d %9d %7d' % (names[l], *row))
 print('# gather role preparing step n+1, relative to the MMA warpgroup entering fc_1 of step n (cycles): start (compositing of n-1 seen), slots refilled,')
 print('#   features gathered (all loads + interpolation done), operand buffer free (colour-layer MMAs of step n retired)')
 for s in range(1, 5):
