@@ -309,24 +309,18 @@ genc_backward_kernel(const float *__restrict__ table, const float *__restrict__ 
             float f[2];
             uint32_t g[2];
 #pragma unroll
-            for (int k = 0; k < 2; k++) {
-                const float x = __fmul_rn(__fadd_rn(genc[k], 1.0f), 0.5f);
-                const float pos = fmaf(x, scale, 0.5f);
-                g[k] = (uint32_t)floorf(pos);
-                f[k] = pos - (float)g[k];
-            }
+            for (int k = 0; k < 2; k++) grid_cell(__fmul_rn(__fadd_rn(genc[k], 1.0f), 0.5f), scale, g[k], f[k]);
             const float *tl = table + ((size_t)level << log2_T) * 8;
 #pragma unroll
             for (int j = 0; j < 4; j++) {
-                const int b3 = j & 1, b4 = j >> 1;
-                const uint32_t K = ((g[0] + b3) * kPrime3) ^ ((g[1] + b4) * kPrime4);
+                const GencCorner c = genc_corner(g, f, j);
                 float v[8];
-                ld8(tl + (size_t)((e ^ K) & mask) * 8, v);
+                ld8(tl + (size_t)((e ^ c.key) & mask) * 8, v);
                 float dot = 0.0f;
 #pragma unroll
-                for (int c = 0; c < 8; c++) dot = fmaf(v[c], d[c], dot);
-                r0 += (b3 ? 1.0f : -1.0f) * (b4 ? f[1] : 1.0f - f[1]) * dot;
-                r1 += (b3 ? f[0] : 1.0f - f[0]) * (b4 ? 1.0f : -1.0f) * dot;
+                for (int k = 0; k < 8; k++) dot = fmaf(v[k], d[k], dot);
+                r0 += ((j & 1) ? 1.0f : -1.0f) * c.w4 * dot;
+                r1 += c.w3 * ((j >> 1) ? 1.0f : -1.0f) * dot;
             }
             r0 *= scale * 0.5f;      // d pos / d genc = scale * d((genc + 1) / 2) / d genc
             r1 *= scale * 0.5f;

@@ -261,32 +261,42 @@ __device__ __forceinline__ void ld8(const float *g, float (&v)[8]) {
     v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
 }
 
-// cell + interpolation fractions of a point on one level of the PRE-BLENDED 3-D table, and the 8 corner
-// (weight, row) pairs -- the arithmetic of encode_level<false> in render_fused.cu, shared with the table backward
+// cell g and interpolation fraction f of coordinate x on a hash-grid level of resolution `scale` (gridencoder.cu:133-140);
+// pos = x*scale + 0.5 is one FFMA in the reference's device code
+__device__ __forceinline__ void grid_cell(float x, float scale, uint32_t &g, float &f) {
+    const float pos = fmaf(x, scale, 0.5f);
+    g = (uint32_t)floorf(pos);
+    f = pos - (float)g;
+}
+
+// table row and trilinear weight of corner i (bit d set: the upper neighbour on dim d) of the 3-D cell (g, f)
+__device__ __forceinline__ uint32_t corner3(uint32_t mask, const uint32_t (&g)[3], const float (&f)[3], uint32_t i, float &w) {
+    const uint32_t b0 = i & 1, b1 = (i >> 1) & 1, b2 = (i >> 2) & 1;
+    w = b0 ? f[0] : 1.0f - f[0];
+    w *= b1 ? f[1] : 1.0f - f[1];
+    w *= b2 ? f[2] : 1.0f - f[2];
+    return ((g[0] + b0) ^ ((g[1] + b1) * kPrime1) ^ ((g[2] + b2) * kPrime2)) & mask;
+}
+
+// corner j (bit 0: upper neighbour on dim 3, bit 1: on dim 4) of the cell (g, f) of the two constant encoder dims: its hash
+// key (a 5-D corner's row is the 3-D corner's row ^ key) and its weight factors on dims 3 and 4
+struct GencCorner { uint32_t key; float w3, w4; };
+__device__ __forceinline__ GencCorner genc_corner(const uint32_t (&g)[2], const float (&f)[2], uint32_t j) {
+    const uint32_t b3 = j & 1, b4 = j >> 1;
+    return {((g[0] + b3) * kPrime3) ^ ((g[1] + b4) * kPrime4), b3 ? f[0] : 1.0f - f[0], b4 ? f[1] : 1.0f - f[1]};
+}
+
+// the 8 corner (weight, row) pairs of a point on one level of the PRE-BLENDED 3-D table -- the corners the forward
+// gather (encode_level in render_fused.cu) reads, for the table backward
 struct Corners3 { float w[8]; uint32_t idx[8]; };
 __device__ __forceinline__ Corners3 corners3(uint32_t mask, float scale, const float (&x)[3]) {
     float f[3];
     uint32_t g[3];
 #pragma unroll
-    for (int d = 0; d < 3; d++) {
-        const float pos = fmaf(x[d], scale, 0.5f);
-        const float fl = floorf(pos);
-        g[d] = (uint32_t)fl;
-        f[d] = pos - (float)g[d];
-    }
-    const uint32_t h0[2] = {g[0], g[0] + 1u};
-    const uint32_t h1[2] = {g[1] * kPrime1, (g[1] + 1u) * kPrime1};
-    const uint32_t h2[2] = {g[2] * kPrime2, (g[2] + 1u) * kPrime2};
+    for (int d = 0; d < 3; d++) grid_cell(x[d], scale, g[d], f[d]);
     Corners3 c;
 #pragma unroll
-    for (int i = 0; i < 8; i++) {
-        const int b0 = i & 1, b1 = (i >> 1) & 1, b2 = (i >> 2) & 1;
-        float w = b0 ? f[0] : 1.0f - f[0];
-        w *= b1 ? f[1] : 1.0f - f[1];
-        w *= b2 ? f[2] : 1.0f - f[2];
-        c.w[i] = w;
-        c.idx[i] = (h0[b0] ^ h1[b1] ^ h2[b2]) & mask;
-    }
+    for (int i = 0; i < 8; i++) c.idx[i] = corner3(mask, g, f, i, c.w[i]);
     return c;
 }
 

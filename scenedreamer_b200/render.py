@@ -273,42 +273,16 @@ def render_rays_forward(voxel_id, depth2, raydirs, cam_ori, global_enc, voxel_di
     rdp = torch.empty(N, H, W, S, 1, dtype=torch.float32, device=dev) if want_samples else None
     Lb = _lib.lib()
     ws = torch.empty(int(Lb.sdb_render_workspace_bytes(N, H, W)), dtype=torch.uint8, device=dev)
-    cam_by_value = None
-    if not cam_ori.is_cuda and N == 1:
-        cam_by_value = [float(v) for v in cam_ori.reshape(3)]       # host pose -> kernel arguments, no H2D copy to wait for
-    else:
-        cam_ori = cam_ori.to(dev, torch.float32).reshape(N, 3).contiguous()
     genc = global_enc.to(dev, torch.float32).reshape(N, 2).contiguous()
-    if uniforms is None:
-        frac = deterministic_fractions(S, dev)
-    else:
-        frac = stratified_offsets(S, dev)
-        uniforms = uniforms.to(dev, torch.float32).reshape(N * H * W, S + 1).contiguous()
     lut = label_lut.to(dev, torch.int32).contiguous()
-    prm = _RenderParams()
-    prm.n_img, prm.H, prm.W, prm.M, prm.S = N, H, W, M, S
-    prm.d_voxel_id, prm.d_depth2, prm.d_raydirs = _ptr(voxel_id), _ptr(depth2), _ptr(raydirs)
-    if cam_by_value is None:
-        prm.d_cam_ori = _ptr(cam_ori)
-    else:
-        prm.d_cam_ori, prm.cam_ori_value = None, (ctypes.c_float * 3)(*cam_by_value)
-    prm.voxel_dims = (ctypes.c_float * 3)(*[float(v) for v in voxel_dims])
-    prm.d_global_enc = _ptr(genc)
-    prm.sample_depth, prm.dists_scale = float(sample_depth), float(dists_scale)
-    prm.d_fractions, prm.d_uniforms = _ptr(frac), _ptr(uniforms)
-    prm.d_label_lut, prm.n_lut = _ptr(lut), int(lut.numel())
-    prm.d_table, prm.d_table3 = _ptr(table), _ptr(table3)
-    prm.L, prm.log2_T, prm.level_S, prm.base_res = int(L), int(log2_T), float(np.log2(per_level_scale)), int(base_res)
-    prm.d_mlp_pack = _ptr(mlp_pack)
-    prm.mlp_pack_stride = int(mlp_pack.stride(0)) if (mlp_pack.dim() == 2 and mlp_pack.shape[0] > 1) else 0
-    prm.precision = int(precision)
     sky = sky.reshape(N, H, W, 64)
     sky_avg = sky_avg.to(dev, torch.float32).reshape(N, 64).contiguous()
-    prm.d_sky, prm.d_sky_avg = _ptr(sky), _ptr(sky_avg)
-    prm.d_net_out, prm.d_depth_out, prm.d_total_weight = _ptr(net_out), _ptr(depth), _ptr(tw)
-    prm.d_weights_out, prm.d_rand_depth_out = _ptr(wts), _ptr(rdp)
-    prm.d_workspace = _ptr(ws)
-    prm.early_stop_transmittance = float(EARLY_STOP_T if early_stop is None else early_stop)
+    prm, keep = _RenderParams(), []
+    _fill_render_params(prm, keep, voxel_id, depth2, raydirs, cam_ori, genc, voxel_dims, lut, mlp_pack, sky, sky_avg,
+                        table=table, table3=table3, S=S, sample_depth=sample_depth, dists_scale=dists_scale, uniforms=uniforms,
+                        precision=precision, per_level_scale=per_level_scale, base_res=base_res, log2_T=log2_T, L=L,
+                        net_out=net_out, depth=depth, tw=tw, wts=wts, rdp=rdp, ws=ws,
+                        early_stop=EARLY_STOP_T if early_stop is None else early_stop)
     with torch.cuda.device(dev):
         code = Lb.sdb_render_rays_forward(ctypes.byref(prm), _stream(dev))
     _lib.check(code, 'sdb_render_rays_forward')
@@ -438,10 +412,12 @@ class _RenderGrads(ctypes.Structure):
     ]
 
 
-def _fill_render_params(prm, keep, voxel_id, depth2, raydirs, cam_ori, genc, voxel_dims, lut, mlp_pack, sky, sky_avg, table3,
-                        S, sample_depth, dists_scale, uniforms, precision, per_level_scale, base_res, log2_T, L, net_out,
-                        depth, tw, wts, rdp, ws):
-    """Fills an sdb_render_params for the pre-blended-table path; `keep` collects tensors that must outlive the call."""
+def _fill_render_params(prm, keep, voxel_id, depth2, raydirs, cam_ori, genc, voxel_dims, lut, mlp_pack, sky, sky_avg, *,
+                        table=None, table3=None, S, sample_depth, dists_scale, uniforms, precision, per_level_scale, base_res,
+                        log2_T, L, net_out, depth, tw, wts, rdp, ws, early_stop=0.0):
+    """Fills an sdb_render_params over the raw `table` or the pre-blended `table3` (the other is None); `keep` collects
+    tensors that must outlive the call.  A host-side camera origin of a single view is passed by value (no H2D copy to wait
+    for); any other goes to the device.  A 2-D `mlp_pack` of several rows holds one pack per image."""
     dev = voxel_id.device
     N, H, W, M = voxel_id.shape[:4]
     if uniforms is None:
@@ -449,20 +425,25 @@ def _fill_render_params(prm, keep, voxel_id, depth2, raydirs, cam_ori, genc, vox
     else:
         frac = stratified_offsets(S, dev)
         uniforms = uniforms.to(dev, torch.float32).reshape(N * H * W, S + 1).contiguous()
-    keep += [frac, uniforms]
     prm.n_img, prm.H, prm.W, prm.M, prm.S = N, H, W, M, S
     prm.d_voxel_id, prm.d_depth2, prm.d_raydirs = _ptr(voxel_id), _ptr(depth2), _ptr(raydirs)
-    prm.d_cam_ori = _ptr(cam_ori)
+    if not cam_ori.is_cuda and N == 1:
+        prm.d_cam_ori, prm.cam_ori_value = None, (ctypes.c_float * 3)(*[float(v) for v in cam_ori.reshape(3)])
+    else:
+        cam_ori = cam_ori.to(dev, torch.float32).reshape(N, 3).contiguous()
+        prm.d_cam_ori = _ptr(cam_ori)
+    keep += [frac, uniforms, cam_ori]
     prm.voxel_dims = (ctypes.c_float * 3)(*[float(v) for v in voxel_dims])
     prm.d_global_enc = _ptr(genc)
     prm.sample_depth, prm.dists_scale = float(sample_depth), float(dists_scale)
     prm.d_fractions, prm.d_uniforms = _ptr(frac), _ptr(uniforms)
     prm.d_label_lut, prm.n_lut = _ptr(lut), int(lut.numel())
-    prm.d_table, prm.d_table3 = None, _ptr(table3)
+    prm.d_table, prm.d_table3 = _ptr(table), _ptr(table3)
     prm.L, prm.log2_T, prm.level_S, prm.base_res = int(L), int(log2_T), float(np.log2(per_level_scale)), int(base_res)
     prm.d_mlp_pack = _ptr(mlp_pack)
-    prm.mlp_pack_stride = 0
+    prm.mlp_pack_stride = int(mlp_pack.stride(0)) if (mlp_pack.dim() == 2 and mlp_pack.shape[0] > 1) else 0
     prm.precision = int(precision)
+    prm.early_stop_transmittance = float(early_stop)
     prm.d_sky, prm.d_sky_avg = _ptr(sky), _ptr(sky_avg)
     prm.d_net_out, prm.d_depth_out, prm.d_total_weight = _ptr(net_out), _ptr(depth), _ptr(tw)
     prm.d_weights_out, prm.d_rand_depth_out = _ptr(wts), _ptr(rdp)
@@ -512,8 +493,10 @@ class _FusedRenderTrainFn(torch.autograd.Function):
             record = _take_scratch(L.sdb_render_train_record_bytes(N, H, W, S), dev, 'record')
             prm, keep = _RenderParams(), []
             _fill_render_params(prm, keep, voxel_id, depth2, raydirs, cam_ori, genc_, cfg['voxel_dims'], lut, pack, sky_, sky_avg_,
-                                table3, S, cfg['sample_depth'], cfg['dists_scale'], cfg.get('uniforms'), prec,
-                                cfg['per_level_scale'], cfg['base_res'], cfg['log2_T'], cfg['L'], net_out, depth, tw, wts, rdp, ws)
+                                table3=table3, S=S, sample_depth=cfg['sample_depth'], dists_scale=cfg['dists_scale'],
+                                uniforms=cfg.get('uniforms'), precision=prec, per_level_scale=cfg['per_level_scale'],
+                                base_res=cfg['base_res'], log2_T=cfg['log2_T'], L=cfg['L'], net_out=net_out, depth=depth, tw=tw,
+                                wts=wts, rdp=rdp, ws=ws)
             _lib.check(L.sdb_render_rays_train_forward(ctypes.byref(prm), _ptr(record), _stream(dev)),
                        'sdb_render_rays_train_forward')
         ctx.cfg, ctx.prm, ctx.keep = cfg, prm, keep + [cam_ori, lut, pack, table3, net_out, depth, tw, wts, rdp, ws, genc_, sky_,
