@@ -341,7 +341,8 @@ int sdb_sky_backward(int32_t n_img, int32_t H, int32_t W, const void *d_record, 
  *         conv4a, conv4b [256,256,1,1]+[256]; conv4 [3,256,1,1]+[3];
  *   d_mod [4][256] = fc_z_cond(z) for ONE style code (the four `adapt` chunks, gancraft_base.py:208-209);
  *   d_net_out [H][W][64] fp32 (the fused kernel's net_out) -> d_rgb [3][H][W] = tanh(raw), d_rgb_raw
- *   [3][H][W] or NULL;  precision 2 = fp16 hi/lo split x3 (fp32-grade, parity), 0 = one fp16 pass;
+ *   [3][H][W] or NULL;  precision 2 = fp16 hi/lo split x3 (fp32-grade, parity), 0 = one fp16 pass
+ *   (sdb_cnn_pack also makes the bf16 x3 pack, precision 1, of the training block below);
  *   d_workspace: sdb_cnn_workspace_bytes() bytes; workspace_ready = 0 on the first call for a given
  *   (workspace, H, W, precision) -- the call then clears the zero borders -- and 1 afterwards.
  * ------------------------------------------------------------------------------------------ */
@@ -354,6 +355,46 @@ int64_t sdb_cnn_workspace_bytes(int32_t H, int32_t W, int32_t precision);
 int sdb_cnn_forward(const float *d_net_out, int32_t H, int32_t W, const void *d_pack, const float *d_mod,
                     int32_t precision, float *d_rgb, float *d_rgb_raw, void *d_workspace, int32_t workspace_ready,
                     void *stream);
+
+/* --------------------------------------------------------------------------------------------
+ * f1 under autograd: RenderCNN + tanh with its backward, bf16 hi/lo split x3 throughout (fp32-grade;
+ * bf16 keeps fp32's exponent range, which the gradients of a mean loss need).
+ *   sdb_cnn_train_forward = sdb_cnn_forward on a pack made with precision 1 that also writes a RECORD
+ *   (sdb_cnn_train_record_bytes(H, W) bytes, one per view): every layer output, the pre-modulation sums
+ *   of the two modulated blocks, and rgb.  The call clears the record's zero borders itself.
+ *   sdb_cnn_backward turns dL/d rgb and/or dL/d rgb_raw ([3][H][W] each, either may be NULL, not both)
+ *   into what torch.autograd gives for RenderCNN + tanh (gancraft_base.py:201-225, :598-601): the
+ *   data-gradient chain on the forward's conv engine with transposed, tap-flipped weights
+ *   (sdb_cnn_pack_backward from the 7 conv weights, state-dict shapes), and the weight gradients on
+ *   the tensor cores (pixels as the reduction dimension).  d_pack (precision 1) and d_mod must be
+ *   those of the recorded forward.  Every non-NULL output of sdb_cnn_grads is written (not
+ *   accumulated into); a NULL output is skipped, with its weight-gradient launch.
+ * Every call is asynchronous on `stream`.
+ * ------------------------------------------------------------------------------------------ */
+int64_t sdb_cnn_train_record_bytes(int32_t H, int32_t W);
+int sdb_cnn_train_forward(const float *d_net_out, int32_t H, int32_t W, const void *d_pack, const float *d_mod,
+                          float *d_rgb, float *d_rgb_raw, void *d_record, void *stream);
+int64_t sdb_cnn_backward_pack_bytes(void);
+int sdb_cnn_pack_backward(const float *d_w1, const float *d_w2a, const float *d_w2b, const float *d_w3a,
+                          const float *d_w3b, const float *d_w4a, const float *d_w4b, void *d_pack, void *stream);
+int64_t sdb_cnn_backward_workspace_bytes(int32_t H, int32_t W);
+
+typedef struct sdb_cnn_grads {
+    float *d_grad_net_out;         /* [H][W][64] dL/d net_out (NHWC, the layout of the fused kernel's net_out) */
+    float *d_grad_mod;             /* [4][256]   dL/d fc_z_cond(z), the four `adapt` chunks                  */
+    float *d_grad_w1, *d_grad_b1;  /* conv1  [256,64,1,1], [256]                                           */
+    float *d_grad_w2a, *d_grad_b2a;/* conv2a [256,256,3,3], [256]                                          */
+    float *d_grad_w2b;             /* conv2b [256,256,3,3]                                                 */
+    float *d_grad_w3a, *d_grad_b3a;/* conv3a [256,256,3,3], [256]                                          */
+    float *d_grad_w3b;             /* conv3b [256,256,3,3]                                                 */
+    float *d_grad_w4a, *d_grad_b4a;/* conv4a [256,256,1,1], [256]                                          */
+    float *d_grad_w4b, *d_grad_b4b;/* conv4b [256,256,1,1], [256]                                          */
+    float *d_grad_w4, *d_grad_b4;  /* conv4  [3,256,1,1], [3]                                              */
+} sdb_cnn_grads;
+
+int sdb_cnn_backward(int32_t H, int32_t W, const void *d_record, const float *d_grad_rgb, const float *d_grad_rgb_raw,
+                     const void *d_bwd_pack, const void *d_pack, const float *d_mod, const sdb_cnn_grads *g,
+                     void *d_workspace, void *stream);
 
 /* --------------------------------------------------------------------------------------------
  * a8 (training): the style modulation of LightningMLP's five ModLinear layers for ONE style code, folded into plain
@@ -416,6 +457,10 @@ int64_t sdb_launch_count(void);
 
 /* Diagnostics only: byte offsets inside the training record / backward workspace (20 int64, see render_train.cu). */
 int sdb_debug_train_layout(int32_t n_img, int32_t H, int32_t W, int32_t S, int32_t L, int32_t log2_T, int64_t *out);
+
+/* Diagnostics only: layout of the RenderCNN training record (14 int64: Hp, Wp, the byte offsets of the
+ * x, y1, t1, u2, y2, t2, u3, y3, t3, y4 bf16 plane pairs and of rgb, the total; see rendercnn.cu).  */
+int sdb_cnn_debug_record_layout(int32_t H, int32_t W, int64_t *out);
 
 /* Diagnostics only: host-mapped (pinned) int32[64] progress buffer written by CTA 0 of the fused
  * kernels (role, step, layer markers); pass NULL to disable (default).                          */

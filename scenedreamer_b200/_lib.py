@@ -69,6 +69,13 @@ SIGNATURES = {
     'sdb_cnn_pack': (c_int, [c_void_p] * 14 + [c_i32, c_void_p, c_void_p]),
     'sdb_cnn_workspace_bytes': (c_i64, [c_i32, c_i32, c_i32]),
     'sdb_cnn_forward': (c_int, [c_void_p, c_i32, c_i32, c_void_p, c_void_p, c_i32, c_void_p, c_void_p, c_void_p, c_i32, c_void_p]),
+    'sdb_cnn_train_record_bytes': (c_i64, [c_i32, c_i32]),
+    'sdb_cnn_train_forward': (c_int, [c_void_p, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'sdb_cnn_backward_pack_bytes': (c_i64, []),
+    'sdb_cnn_pack_backward': (c_int, [c_void_p] * 9),
+    'sdb_cnn_backward_workspace_bytes': (c_i64, [c_i32, c_i32]),
+    'sdb_cnn_backward': (c_int, [c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                 c_void_p]),
     'sdb_adam_step': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, ctypes.c_double, ctypes.c_double, ctypes.c_double,
                               ctypes.c_double, c_i64, c_void_p]),
     'sdb_pose_stats_workspace_bytes': (c_i64, [c_i32]),
@@ -78,6 +85,7 @@ SIGNATURES = {
     'sdb_world_truncate': (c_int, [c_void_p, c_i32, c_i32, c_i32, c_i32, c_void_p, c_void_p]),
     'sdb_launch_count': (c_i64, []),
     'sdb_debug_train_layout': (c_int, [c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, ctypes.POINTER(c_i64)]),
+    'sdb_cnn_debug_record_layout': (c_int, [c_i32, c_i32, ctypes.POINTER(c_i64)]),
     'sdb_debug_set_progress_buffer': (None, [c_void_p]),
     'sdb_modulate_forward': (c_int, [ctypes.POINTER(c_void_p), c_void_p, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p]),
     'sdb_modulate_backward': (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p,

@@ -79,7 +79,8 @@ class _FusedState:
         self.cnn, self.cnn_key, self.cnn_precision = None, None, rendercnn.PRECISION_FP16X3
         self.frame = _FrameCache()
         self.stats = {'fused_calls': 0, 'frame_launches': 0, 'tile_hits': 0, 'train_calls': 0, 'reference_calls': 0,
-                      'cnn_frame_launches': 0, 'cnn_tile_hits': 0, 'cnn_calls': 0, 'cnn_reference_calls': 0}
+                      'cnn_frame_launches': 0, 'cnn_tile_hits': 0, 'cnn_calls': 0, 'cnn_reference_calls': 0,
+                      'cnn_train_calls': 0}
 
     @property
     def lut(self):
@@ -310,18 +311,23 @@ def fused_forward_global(self, net_out, z):
     cores.  When `net_out` is a tile of the frame the fused per-pixel launch produced (the unmodified tile loop of
     inference_givenstyle), the CNN runs ONCE on the whole padded frame and every tile gets its window: the receptive
     radius is 4 px, the loop crops pad/2 = 15 px from every tile side (DESIGN.md section 1).  Calls that need gradients
-    through the CNN (gen_update) keep the reference's cuDNN composition."""
+    through the CNN (gen_update) run the recording bf16 x3 forward, whose backward is the library's as well
+    (rendercnn._RenderCNNTrainFn); under autocast they keep the reference's composition."""
     st = _state(self)
     reference = type(self)._sdb200_reference_forward_global
     needs_grad = torch.is_grad_enabled() and (net_out.requires_grad or (z is not None and z.requires_grad) or
                                               any(q.requires_grad for q in self.denoiser.parameters()))
     eng = None
-    if enabled() and os.environ.get('SDB200_CNN', '1') != '0' and not needs_grad and z is not None and net_out.is_cuda and \
-            net_out.dim() == 4 and net_out.shape[-1] == 64 and net_out.dtype == torch.float32:
+    if enabled() and os.environ.get('SDB200_CNN', '1') != '0' and z is not None and net_out.is_cuda and \
+            net_out.dim() == 4 and net_out.shape[-1] == 64 and net_out.dtype == torch.float32 and \
+            not (needs_grad and torch.is_autocast_enabled()):
         eng = st.get_cnn(self)
     if eng is None:
         st.stats['cnn_reference_calls'] += 1
         return reference(self, net_out, z)
+    if needs_grad:
+        st.stats['cnn_train_calls'] += 1
+        return eng.forward_train(net_out, z, {'denoiser.' + k: v for k, v in self.denoiser.named_parameters()})
     full = st.frame.out
     if full is not None and net_out.shape[0] == 1 and z.shape[0] == 1:
         base = full['net_out']

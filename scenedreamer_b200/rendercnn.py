@@ -1,4 +1,5 @@
-"""Host side of the tensor-core RenderCNN (libsdb200: sdb_cnn_pack / sdb_cnn_forward).
+"""Host side of the tensor-core RenderCNN (libsdb200: sdb_cnn_pack / sdb_cnn_forward, and under autograd
+sdb_cnn_train_forward / sdb_cnn_backward).
 
 Mirrors Base3DGenerator._forward_global (imaginaire/generators/gancraft_base.py:588-603): per-pixel feature map
 [N,H,W,64] + style code -> (tanh image, raw image) [N,3,H,W], with RenderCNN.forward (:201-225) evaluated once on the
@@ -12,6 +13,7 @@ import torch.nn.functional as F
 from . import _lib
 
 PRECISION_FP16 = 0      # one fp16 pass per product (the class of the reference's default, cuDNN TF32)
+PRECISION_BF16X3 = 1    # bf16 hi/lo split, 3 passes: the training forward and backward (gradients need bf16's range)
 PRECISION_FP16X3 = 2    # fp16 hi/lo split, 3 passes: fp32-grade (parity default)
 
 _NAMES = ('conv1.weight', 'conv1.bias', 'conv2a.weight', 'conv2a.bias', 'conv2b.weight', 'conv3a.weight', 'conv3a.bias',
@@ -36,6 +38,82 @@ def supported(P, prefix='denoiser.'):
         if t is None or len(t.shape) != len(shp) or any(a is not None and a != b for a, b in zip(shp, t.shape)):
             return False
     return True
+
+
+_CONV_W = ('conv1.weight', 'conv2a.weight', 'conv2b.weight', 'conv3a.weight', 'conv3b.weight', 'conv4a.weight', 'conv4b.weight')
+
+
+class _RenderCNNTrainFn(torch.autograd.Function):
+    """(net_out [N,H,W,64], mod [N or 1,4,256], the 14 denoiser tensors in _NAMES order) -> (rgb, raw) [N,3,H,W].
+    The forward packs the weights (bf16 x3) and keeps one record per view; the backward runs sdb_cnn_backward per view
+    and releases the records."""
+
+    @staticmethod
+    def forward(ctx, net_out, mod, *params):
+        L = _lib.lib()
+        dev = net_out.device
+        N, H, W = net_out.shape[:3]
+        x = net_out.detach().contiguous()
+        m = mod.detach().to(torch.float32).contiguous()
+        ws = [t.detach().to(torch.float32).contiguous() for t in params]
+        rgb = torch.empty(N, 3, H, W, dtype=torch.float32, device=dev)
+        raw = torch.empty(N, 3, H, W, dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            pack = torch.empty(int(L.sdb_cnn_pack_bytes(PRECISION_BF16X3)), dtype=torch.uint8, device=dev)
+            _lib.check(L.sdb_cnn_pack(*[_ptr(t) for t in ws], PRECISION_BF16X3, _ptr(pack), _stream(dev)), 'sdb_cnn_pack')
+            records = []
+            for i in range(N):
+                rec = torch.empty(int(L.sdb_cnn_train_record_bytes(H, W)), dtype=torch.uint8, device=dev)
+                _lib.check(L.sdb_cnn_train_forward(_ptr(x[i]), H, W, _ptr(pack), _ptr(m[i if m.shape[0] > 1 else 0]), _ptr(rgb[i]),
+                                                   _ptr(raw[i]), _ptr(rec), _stream(dev)), 'sdb_cnn_train_forward')
+                records.append(rec)
+        ctx.records, ctx.pack, ctx.mod, ctx.ws = records, pack, m, ws
+        return rgb, raw
+
+    @staticmethod
+    def backward(ctx, g_rgb, g_raw):
+        if ctx.records is None:
+            raise RuntimeError('RenderCNN: the training record of this pass was released by its first backward '
+                               '(retain_graph / double backward are not supported on the tensor-core path)')
+        L = _lib.lib()
+        records, pack, m, ws = ctx.records, ctx.pack, ctx.mod, ctx.ws
+        ctx.records = None
+        dev = pack.device
+        N = len(records)
+        H, W = (g_rgb if g_rgb is not None else g_raw).shape[2:]
+        need_x, need_m = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        need_p = ctx.needs_input_grad[2:]
+        g_rgb = g_rgb.to(torch.float32).contiguous() if g_rgb is not None else None
+        g_raw = g_raw.to(torch.float32).contiguous() if g_raw is not None else None
+        g_x = torch.empty(N, H, W, 64, dtype=torch.float32, device=dev) if need_x else None
+        g_m = torch.empty(N, 4, 256, dtype=torch.float32, device=dev) if need_m else None
+        g_p = [torch.zeros_like(w) if need else None for w, need in zip(ws, need_p)]
+        with torch.cuda.device(dev):
+            bpack = torch.empty(int(L.sdb_cnn_backward_pack_bytes()), dtype=torch.uint8, device=dev)
+            conv_w = [ws[_NAMES.index(n)] for n in _CONV_W]
+            _lib.check(L.sdb_cnn_pack_backward(*[_ptr(t) for t in conv_w], _ptr(bpack), _stream(dev)), 'sdb_cnn_pack_backward')
+            work = torch.empty(int(L.sdb_cnn_backward_workspace_bytes(H, W)), dtype=torch.uint8, device=dev)
+            view_p = [torch.empty_like(t) if t is not None else None for t in g_p] if N > 1 else g_p
+            for i in range(N):
+                grads = _CnnGrads(_ptr(g_x[i]) if need_x else None, _ptr(g_m[i]) if need_m else None,
+                                  *[_ptr(t) for t in view_p])
+                _lib.check(L.sdb_cnn_backward(H, W, _ptr(records[i]), _ptr(g_rgb[i]) if g_rgb is not None else None,
+                                              _ptr(g_raw[i]) if g_raw is not None else None, _ptr(bpack), _ptr(pack),
+                                              _ptr(m[i if m.shape[0] > 1 else 0]), ctypes.byref(grads), _ptr(work), _stream(dev)),
+                           'sdb_cnn_backward')
+                if N > 1:
+                    for acc, v in zip(g_p, view_p):
+                        if acc is not None:
+                            acc.add_(v)
+        if g_m is not None and m.shape[0] == 1 and N > 1:
+            g_m = g_m.sum(0, keepdim=True)
+        return (g_x, g_m) + tuple(g_p)
+
+
+class _CnnGrads(ctypes.Structure):
+    """sdb_cnn_grads (include/sdb200.h): dL/dnet_out, dL/dmod, then the 14 parameter gradients in _NAMES order."""
+    _fields_ = [('d_grad_net_out', ctypes.c_void_p), ('d_grad_mod', ctypes.c_void_p)] + \
+               [('d_grad_' + n.replace('.weight', '_w').replace('.bias', '_b'), ctypes.c_void_p) for n in _NAMES]
 
 
 class RenderCNNEngine:
@@ -67,6 +145,16 @@ class RenderCNNEngine:
         """fc_z_cond(z) -> [N, 4, 256]: (w, b) of the two modulated blocks (gancraft_base.py:208-209)."""
         p = self.prefix
         return F.linear(z, self.P[p + 'fc_z_cond.weight'], self.P[p + 'fc_z_cond.bias']).reshape(z.shape[0], 4, 256).contiguous()
+
+    def forward_train(self, net_out, z, P):
+        """Differentiable forward for the training step: P maps the same `denoiser.*` names to the LIVE Parameters
+        (state_dict() hands out detached aliases, so self.P cannot carry gradients).  The modulation fc_z_cond(z) is
+        torch's own F.linear, so z, fc_z_cond.weight and .bias get their gradients from autograd."""
+        if not net_out.is_cuda or net_out.dtype != torch.float32 or net_out.dim() != 4 or net_out.shape[-1] != 64:
+            raise RuntimeError('net_out must be a float32 CUDA tensor [N,H,W,64]')
+        p = self.prefix
+        mod = F.linear(z.to(net_out.device, torch.float32), P[p + 'fc_z_cond.weight'], P[p + 'fc_z_cond.bias'])
+        return _RenderCNNTrainFn.apply(net_out, mod.reshape(z.shape[0], 4, 256), *[P[p + n] for n in _NAMES])
 
     def forward(self, net_out, z, want_raw=True):
         """net_out [N,H,W,64] fp32 CUDA, z [N,256] (or [1,256]) -> (fake_images [N,3,H,W], fake_images_raw or None)."""
