@@ -311,6 +311,25 @@ typedef struct sdb_render_grads {
 int64_t sdb_render_backward_workspace_bytes(int32_t n_img, int32_t H, int32_t W, int32_t S, int32_t L, int32_t log2_T);
 int sdb_render_rays_backward(const sdb_render_params *p, const void *d_record, const sdb_render_grads *g, void *stream);
 
+/* A batch of views of ONE scene in one recorded pass.  sdb_render_rays_train_forward takes n_img >= 1 views: one pack per
+ * view through mlp_pack_stride (0 = shared; else >= sdb_mlp_pack_bytes(2)), d_sky_avg [n_img, 64], and d_table3 of the one
+ * scene code all views share (the caller checks that their global_enc are equal).  Its record
+ * (sdb_render_train_record_bytes(n_img, ...)) lists the live tiles grouped by image and keeps per image {first list
+ * position, live tiles} in its header, on the device; with n_img == 1 its layout is the single-view one.
+ * sdb_render_rays_backward_views differentiates such a record: the fields of `g` are those of sdb_render_grads, with one
+ * backward pack per view through bwd_pack_stride (0 = shared; else >= sdb_mlp_backward_pack_bytes()) and the gradients of
+ * view i at the given strides (floats; >= one view's size when n_img > 1): d_grad_w1ext + i * w1ext_stride, d_grad_wh +
+ * i * wh_stride, d_grad_wsig + i * wsig_stride, d_grad_wout + i * wout_stride, d_grad_sky_avg + i * sky_avg_stride.  The
+ * weight gradients are per view (W' = W * alpha(z_i) differs per style code); d_grad_table and d_grad_global_enc are
+ * summed over the views.  The views are taken one at a time over ONE view-sized workspace:
+ * sdb_render_backward_workspace_bytes(n_img, ...) is the one-view size for every n_img.  The table transpose and the
+ * scene-code gradient run once per batch.  sdb_render_rays_backward is this call for n_img == 1.                   */
+typedef struct sdb_render_view_grads {
+    sdb_render_grads g;
+    int64_t w1ext_stride, wh_stride, wsig_stride, wout_stride, sky_avg_stride;
+} sdb_render_view_grads;
+int sdb_render_rays_backward_views(const sdb_render_params *p, const void *d_record, const sdb_render_view_grads *g, void *stream);
+
 /* --------------------------------------------------------------------------------------------
  * a9 under autograd.  sdb_sky_train_forward = sdb_sky_forward (fp16x3, ONE style code / image)
  * that also records PE(raydir), the five hidden activations (bf16) and their LeakyReLU sign
@@ -330,6 +349,23 @@ int64_t sdb_sky_backward_workspace_bytes(int32_t n_img, int32_t H, int32_t W);
 int sdb_sky_backward(int32_t n_img, int32_t H, int32_t W, const void *d_record, const float *d_grad_sky,
                      const void *d_bwd_pack, float *d_grad_w1ext, float *d_grad_wh, float *d_grad_wout,
                      void *d_workspace, void *stream);
+
+/* The sky branch of a batch of views: sdb_sky_train_forward_views records n_img views with one pack per view
+ * (pack_stride bytes; 0 = shared, else >= sdb_sky_pack_bytes(2)); sdb_sky_backward_views returns each view's SKYMLP
+ * gradients at the given strides (floats; >= one view's size when n_img > 1), one backward pack per view through
+ * bwd_pack_stride (0 = shared, else >= sdb_sky_backward_pack_bytes()).  The views are taken one at a time over ONE
+ * view-sized workspace: sdb_sky_backward_workspace_bytes(n_img, ...) is the one-view size for every n_img.          */
+typedef struct sdb_sky_view_grads {
+    float *d_grad_w1ext; int64_t w1ext_stride;
+    float *d_grad_wh;    int64_t wh_stride;
+    float *d_grad_wout;  int64_t wout_stride;
+} sdb_sky_view_grads;
+int sdb_sky_train_forward_views(const float *d_raydirs, int32_t n_img, int32_t H, int32_t W, const void *d_sky_pack,
+                                int64_t pack_stride, float *d_sky, float *d_sky_avg, void *d_workspace, void *d_record,
+                                void *stream);
+int sdb_sky_backward_views(int32_t n_img, int32_t H, int32_t W, const void *d_record, const float *d_grad_sky,
+                           const void *d_bwd_pack, int64_t bwd_pack_stride, const sdb_sky_view_grads *g,
+                           void *d_workspace, void *stream);
 
 /* --------------------------------------------------------------------------------------------
  * f1. RenderCNN + tanh on the tensor cores: per-pixel feature map -> image.

@@ -65,6 +65,10 @@ SIGNATURES = {
     'sdb_sky_backward_workspace_bytes': (c_i64, [c_i32, c_i32, c_i32]),
     'sdb_sky_backward': (c_int, [c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                  c_void_p]),
+    'sdb_render_rays_backward_views': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    'sdb_sky_train_forward_views': (c_int, [c_void_p, c_i32, c_i32, c_i32, c_void_p, c_i64, c_void_p, c_void_p, c_void_p, c_void_p,
+                                            c_void_p]),
+    'sdb_sky_backward_views': (c_int, [c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_void_p, c_void_p]),
     'sdb_cnn_pack_bytes': (c_i64, [c_i32]),
     'sdb_cnn_pack': (c_int, [c_void_p] * 14 + [c_i32, c_void_p, c_void_p]),
     'sdb_cnn_workspace_bytes': (c_i64, [c_i32, c_i32, c_i32]),

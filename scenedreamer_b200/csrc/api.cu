@@ -10,10 +10,10 @@ extern "C" int64_t sdb_launch_count(void) { return (int64_t)g_launches.load(std:
 #define SDB_STR2(x) #x
 #define SDB_STR(x) SDB_STR2(x)
 
-extern "C" int sdb_version(void) { return 100; }  // 0.1.0
+extern "C" int sdb_version(void) { return 101; }  // 0.1.1
 
 extern "C" const char *sdb_build_info(void) {
-    return "libsdb200 0.1.0 sm_90a nvcc " SDB_STR(__CUDACC_VER_MAJOR__) "." SDB_STR(__CUDACC_VER_MINOR__)
+    return "libsdb200 0.1.1 sm_90a nvcc " SDB_STR(__CUDACC_VER_MAJOR__) "." SDB_STR(__CUDACC_VER_MINOR__)
            " (wgmma fused render path, no CPU fallback)";
 }
 

@@ -374,6 +374,14 @@ mlp_kernel(const Params p)
     // work item (work_mult = S, one step each), which balances a few hundred tiles over 148 CTAs far better than whole tiles
     const int wmult = (MODE == kBwd && p.work_mult > 1) ? p.work_mult : 1;
     const int n_work = RAYQ ? (int)gridDim.x : (ONE_STEP ? p.n_tiles : *p.n_live * wmult);
+    // the render chain over one image of a multi-view record: its work items start at record item view[0] * wmult (the record
+    // lists live tiles grouped by image); read per work item rather than kept in a register across the roles' loops
+    auto rec_work = [&](int work) {
+        if constexpr (MODE != kBwd) return work;
+        int first;
+        asm volatile("ld.global.nc.s32 %0, [%1];" : "=r"(first) : "l"(p.view));      // volatile: re-read where used, not held
+        return work + first * wmult;
+    };
     constexpr bool STATE = MODE == kRender;      // per-ray sampling state (gather -> epilogue hand-off) exists
     const int S = ONE_STEP ? 1 : p.S;
     const int SL = RAYQ ? 0x3fffffff : S;        // steps of one work item: open-ended for ray slots (ended through sStop)
@@ -462,7 +470,7 @@ mlp_kernel(const Params p)
         for (int it = 0;; it++) {
             const int work = fetch_work(it);
             if (work < 0) break;
-            const int tile = RAYQ ? 0 : (ONE_STEP ? work : p.tile_list[work / wmult]);
+            const int tile = RAYQ ? 0 : (ONE_STEP ? work : p.tile_list[rec_work(work) / wmult]);
             const TileCoord tc = tile_coord(p, tile);
             const int buf = it & 1;
             const float *st = sState + buf * kStFloats * kRows;
@@ -520,7 +528,7 @@ mlp_kernel(const Params p)
                     // through (prefetched before the accumulator wait)
                     uint4 mw = make_uint4(0u, 0u, 0u, 0u);
                     if constexpr (BWD)
-                        mw = __ldg(reinterpret_cast<const uint4 *>(p.tr.mask + ((step_id * kNumAct + (NACT - 1 - l)) * kRows + row) * 8 + half * 4));
+                        mw = __ldg(reinterpret_cast<const uint4 *>(p.tr.mask + (((long long)rec_work(work) * S + s) * kNumAct + (NACT - 1 - l)) * kRows * 8 + row * 8 + half * 4));
                     if ((tid & 127) == 0) SDB_MARK(half, 1, n, l);
                     tc05::mbar_wait(&bars[B_ACC + rb], (n * NH + l) & 1);
                     if ((tid & 127) == 0) SDB_MARK(half, 2, n, l);
@@ -791,7 +799,7 @@ mlp_kernel(const Params p)
       for (int it = 0;; it++) {
           const int work = fetch_work(it);
           if (work < 0) break;
-          const int tile = RAYQ ? 0 : (ONE_STEP ? work : p.tile_list[work / wmult]);
+          const int tile = RAYQ ? 0 : (ONE_STEP ? work : p.tile_list[rec_work(work) / wmult]);
           const uint8_t *pack = p.pack + (long long)tile_coord(p, tile).img * p.pack_stride;
           for (int s = 0; s < SL; s++, n++) {
               if (ESTOP && s >= 2 && s >= sStop[it & 1]) break;
@@ -917,7 +925,7 @@ mlp_kernel(const Params p)
             }
             const int work = fetch_work(it);
             if (work < 0) break;
-            const int tile = RAYQ ? 0 : (ONE_STEP ? work : p.tile_list[work / wmult]);
+            const int tile = RAYQ ? 0 : (ONE_STEP ? work : p.tile_list[rec_work(work) / wmult]);
             const TileCoord tc = tile_coord(p, tile);
             const int y = tc.y0 + (row >> 4), x = tc.x0 + (row & 15);
             const bool valid = (y < p.H) && (x < p.W);
@@ -1171,6 +1179,46 @@ prepass_kernel(const Params p, int32_t *tile_list, int32_t *n_live)
     if (valid) sky_only_ray(p, tc.img, ray);
 }
 
+// ---- training pre-pass: the live-tile list grouped by image, so that the backward can take the record one image at a time.
+// Record header (int32): [0] live tiles of all images, [1 + 2i] first live-list position of image i, [2 + 2i] its live tiles.
+// train_prepass_kernel counts per image and leaves each live tile's rank inside its image in tile_work; train_list_kernel
+// turns the counts into offsets and the ranks into list positions.
+__global__ void __launch_bounds__(kRows)
+train_prepass_kernel(const Params p, int32_t *hdr)
+{
+    const int tile = blockIdx.x, row = threadIdx.x;
+    const TileCoord tc = tile_coord(p, tile);
+    const int y = tc.y0 + (row >> 4), x = tc.x0 + (row & 15);
+    const bool valid = (y < p.H) && (x < p.W);
+    const long long ray = ((long long)tc.img * p.H + y) * p.W + x;
+    const bool live = valid && (__ldg(p.voxel_id + ray * p.M) != 0);
+    if (__syncthreads_or(live ? 1 : 0)) {
+        if (row == 0) p.tr.tile_work[tile] = atomicAdd(hdr + 2 + 2 * tc.img, 1);
+        return;
+    }
+    if (row == 0) p.tr.tile_work[tile] = -1;
+    if (valid) sky_only_ray(p, tc.img, ray);
+}
+
+__global__ void __launch_bounds__(256)
+train_list_kernel(const Params p, int32_t *hdr, int32_t *tile_list)
+{
+    const int tile = blockIdx.x * 256 + threadIdx.x;
+    if (tile == 0) {
+        int first = 0;
+        for (int i = 0; i < p.n_img; i++) { hdr[1 + 2 * i] = first; first += hdr[2 + 2 * i]; }
+        hdr[0] = first;
+    }
+    if (tile >= p.n_tiles) return;
+    const int rank = p.tr.tile_work[tile];
+    if (rank < 0) return;
+    const int img = tile / (p.tiles_x * p.tiles_y);
+    int w = rank;
+    for (int i = 0; i < img; i++) w += hdr[2 + 2 * i];
+    p.tr.tile_work[tile] = w;
+    tile_list[w] = tile;
+}
+
 // ---- pre-pass of the ray-slot kernel: queue of live rays (tile order) + outputs of every ray that hits nothing ----
 __global__ void __launch_bounds__(kRows)
 prepass_rays_kernel(const Params p, int32_t *ray_list, int32_t *n_rays)
@@ -1378,6 +1426,14 @@ int launch_train_forward(const Params &p, int grid, cudaStream_t st) { return la
 int launch_bwd_chain(const Params &p, int grid, cudaStream_t st) { return launch_mlp<1, false, kBwd>(p, grid, st); }
 int launch_sky_train_forward(const Params &p, int grid, cudaStream_t st) { return launch_mlp<2, false, kSky, true>(p, grid, st); }
 int launch_sky_bwd_chain(const Params &p, int grid, cudaStream_t st) { return launch_mlp<1, false, kSkyBwd>(p, grid, st); }
+int launch_train_prepass(const Params &p, int32_t *hdr, int32_t *tile_list, cudaStream_t st) {
+    SDB_CUDA(cudaMemsetAsync(hdr, 0, (size_t)(1 + 2 * p.n_img) * 4, st));
+    train_prepass_kernel<<<p.n_tiles, kRows, 0, st>>>(p, hdr);
+    SDB_CHECK_LAUNCH();
+    train_list_kernel<<<(p.n_tiles + 255) / 256, 256, 0, st>>>(p, hdr, tile_list);
+    SDB_CHECK_LAUNCH();
+    return SDB_OK;
+}
 int launch_prepass(const Params &p, int32_t *ws, cudaStream_t st) {
     SDB_CUDA(cudaMemsetAsync(ws, 0, 16, st));
     prepass_kernel<<<p.n_tiles, kRows, 0, st>>>(p, ws + 4, ws);
@@ -1517,7 +1573,7 @@ static int sky_forward_impl(const float *d_raydirs, int32_t n_img, int32_t H, in
     if (!d_raydirs || !d_sky_pack || !d_sky || !d_sky_avg || !d_workspace) return SDB_EINVAL;
     if (n_img <= 0 || H <= 0 || W <= 0) return SDB_EINVAL;
     if (precision < 0 || precision > 2) return SDB_EUNSUPPORTED;
-    if (d_record && (precision != 2 || n_img != 1)) return SDB_EUNSUPPORTED;
+    if (d_record && precision != 2) return SDB_EUNSUPPORTED;
     cudaStream_t st = (cudaStream_t)stream;
     Params p{};
     p.n_img = n_img; p.H = H; p.W = W; p.M = 1; p.S = 1;
@@ -1562,7 +1618,16 @@ extern "C" int sdb_sky_train_forward(const float *d_raydirs, int32_t n_img, int3
                                      float *d_sky, float *d_sky_avg, void *d_workspace, void *d_record, void *stream)
 {
     if (!d_record) return SDB_EINVAL;
+    if (n_img != 1) return n_img < 1 ? SDB_EINVAL : SDB_EUNSUPPORTED;
     return sky_forward_impl(d_raydirs, n_img, H, W, d_sky_pack, 0, 2, d_sky, d_sky_avg, d_workspace, d_record, stream);
+}
+
+extern "C" int sdb_sky_train_forward_views(const float *d_raydirs, int32_t n_img, int32_t H, int32_t W, const void *d_sky_pack,
+                                           int64_t pack_stride, float *d_sky, float *d_sky_avg, void *d_workspace, void *d_record,
+                                           void *stream)
+{
+    if (!d_record || pack_stride < 0 || (n_img > 1 && pack_stride > 0 && pack_stride < rf::packBytes<rf::kSky>(2))) return SDB_EINVAL;
+    return sky_forward_impl(d_raydirs, n_img, H, W, d_sky_pack, pack_stride, 2, d_sky, d_sky_avg, d_workspace, d_record, stream);
 }
 
 namespace rf {

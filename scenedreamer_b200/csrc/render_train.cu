@@ -21,6 +21,8 @@
 #include <stdio.h>
 #include <stdlib.h>
 
+#include <vector>
+
 #include "rf_common.cuh"
 #include "wgrad.cuh"
 
@@ -29,12 +31,13 @@ namespace rf {
 // ---- record / workspace layouts --------------------------------------------------------------------
 struct RecordLayout { size_t hdr, tile_list, tile_work, rayflags, x3, x0, act, mask, sig, nds, c, total; };
 static size_t align_up(size_t v) { return rf_align_up(v); }
-static RecordLayout record_layout(long long n_tiles, int S) {
+// header: int32 [0] live tiles, then {first live-list position, live tiles} per image (launch_train_prepass); 16 bytes for one image
+static RecordLayout record_layout(int n_img, long long n_tiles, int S) {
     const size_t cap = (size_t)n_tiles * S * kRows, steps = (size_t)n_tiles * S;
     RecordLayout r{};
     size_t o = 0;
-    r.hdr = o; o += 16;
-    r.tile_list = o; o = align_up(o + (size_t)n_tiles * 4);      // directly behind the 16-byte header (prepass contract)
+    r.hdr = o; o += ((size_t)(1 + 2 * n_img) * 4 + 15) / 16 * 16;
+    r.tile_list = o; o = align_up(o + (size_t)n_tiles * 4);
     r.tile_work = o; o = align_up(o + (size_t)n_tiles * 4);
     r.rayflags = o; o = align_up(o + (size_t)n_tiles * kRows * 4);
     r.x3 = o; o = align_up(o + cap * 16);
@@ -100,6 +103,8 @@ composite_backward_kernel(const Params p, const float *__restrict__ g_out, float
                           float *__restrict__ dsky_avg, float *__restrict__ dc32, uint16_t *__restrict__ dc16,
                           float *__restrict__ dsig32, uint16_t *__restrict__ dsig16)
 {
+    // p covers ONE image (n_img 1, its rays and tiles); the record is read at the work item tile_work names, the workspace
+    // (dc*, dsig*) holds only this image's items, which start at record item p.view[0]
     __shared__ float s_avg[8][kOutC];
     const int tile = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const TileCoord tc = tile_coord(p, tile);
@@ -128,6 +133,7 @@ composite_backward_kernel(const Params p, const float *__restrict__ g_out, float
         const uint32_t fl = p.tr.rayflags[(long long)work * kRows + row];
         const bool live = fl & 1u, nosky = fl & 2u, valid = fl & 4u;
         const long long slot0 = (long long)work * S * kRows + row;      // slot of sample s: slot0 + s * 128
+        const long long wofs = (long long)__ldg(p.view) * S * kRows;      // record slot - workspace slot
 
         // ---- phase 1: compositing weights, every lane walks the ray; lane s (and s-32) keeps sample s ----
         float w0 = 0, T0 = 0, e0 = 0, sg0 = 0, nd0 = 0, w1 = 0, T1 = 0, e1 = 0, sg1 = 0, nd1 = 0;
@@ -155,8 +161,8 @@ composite_backward_kernel(const Params p, const float *__restrict__ g_out, float
             const float dw = live ? dot - gsky : 0.0f;
             const float ws = __shfl_sync(full, s < 32 ? w0 : w1, s & 31);
             const float dcx = in_clamp(c.x) ? ws * g.x : 0.0f, dcy = in_clamp(c.y) ? ws * g.y : 0.0f;
-            *reinterpret_cast<float2 *>(dc32 + slot * kOutC + 2 * lane) = make_float2(dcx, dcy);
-            *reinterpret_cast<uint32_t *>(rec_chunk(dc16, slot, kOutC / 8, lane >> 2) + 2 * (lane & 3)) = tc05::pack2<true>(dcx, dcy);
+            *reinterpret_cast<float2 *>(dc32 + (slot - wofs) * kOutC + 2 * lane) = make_float2(dcx, dcy);
+            *reinterpret_cast<uint32_t *>(rec_chunk(dc16, slot - wofs, kOutC / 8, lane >> 2) + 2 * (lane & 3)) = tc05::pack2<true>(dcx, dcy);
             if (s == lane) dw0 = dw;
             if (s == lane + 32) dw1 = dw;
         }
@@ -175,14 +181,14 @@ composite_backward_kernel(const Params p, const float *__restrict__ g_out, float
         if (lane < S) {
             const float de = dw0 * (T0 * expf(-e0)) - ex0;
             const float ds = sg0 > 0.0f ? de * nd0 : 0.0f;
-            const long long slot = slot0 + (long long)lane * kRows;
+            const long long slot = slot0 - wofs + (long long)lane * kRows;
             dsig32[slot] = ds;
             *reinterpret_cast<uint4 *>(dsig16 + slot * 8) = make_uint4(tc05::pack2<true>(ds, 0.0f), 0u, 0u, 0u);
         }
         if (lane + 32 < S) {
             const float de = dw1 * (T1 * expf(-e1)) - ex1;
             const float ds = sg1 > 0.0f ? de * nd1 : 0.0f;
-            const long long slot = slot0 + (long long)(lane + 32) * kRows;
+            const long long slot = slot0 - wofs + (long long)(lane + 32) * kRows;
             dsig32[slot] = ds;
             *reinterpret_cast<uint4 *>(dsig16 + slot * 8) = make_uint4(tc05::pack2<true>(ds, 0.0f), 0u, 0u, 0u);
         }
@@ -220,14 +226,14 @@ __device__ __forceinline__ void red_add8(float *dst, const float (&v)[8]) {
 __global__ void __launch_bounds__(256)
 table3_backward_kernel(const Params p, const float *__restrict__ dx0, float *__restrict__ dt3, int agg_levels)
 {
-    // the number of live slots is read on the device: the host never waits for the forward pass to size a launch
-    const long long n_slots = (long long)__ldg(p.n_live) * p.S * kRows;
-    const long long slot = blockIdx.x * 256ll + threadIdx.x;
+    // the number of live slots of this image is read on the device: the host never waits for the forward pass to size a launch
+    const long long n_slots = (long long)__ldg(p.view + 1) * p.S * kRows;
+    const long long slot = blockIdx.x * 256ll + threadIdx.x;      // of this image (dx0); the record's is slot + view[0] * S * 128
     const int level = blockIdx.y, lane = threadIdx.x & 31;
     const unsigned full = 0xffffffffu;
     bool active = slot < n_slots;
     float4 x = make_float4(0.0f, 0.0f, 0.0f, -1.0f);
-    if (active) x = p.tr.x3[slot];
+    if (active) x = p.tr.x3[(long long)__ldg(p.view) * p.S * kRows + slot];
     active = active && !(x.w < 0.0f);                          // outside the volume / sky-only ray: no table contribution
     float g[8] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
     if (active) {
@@ -354,18 +360,20 @@ static void add_jobs(WgJob *jobs, int &n, const uint16_t *A, int a_cols, const u
 
 }  // namespace rf
 
+// Records of n_img views hold every view's items (grouped by image); the backward takes them one image at a time over ONE
+// view-sized workspace, so its size does not depend on n_img.
+static long long view_tiles(int32_t H, int32_t W) { return (long long)sdb_div_up(H, rf::kTileH) * sdb_div_up(W, rf::kTileW); }
+
 extern "C" int64_t sdb_render_train_record_bytes(int32_t n_img, int32_t H, int32_t W, int32_t S) {
     using namespace rf;
     if (n_img <= 0 || H <= 0 || W <= 0 || S < 1 || S > kMaxS) return 0;
-    const long long n_tiles = (long long)n_img * sdb_div_up(H, kTileH) * sdb_div_up(W, kTileW);
-    return (int64_t)record_layout(n_tiles, S).total;
+    return (int64_t)record_layout(n_img, n_img * view_tiles(H, W), S).total;
 }
 
 extern "C" int64_t sdb_render_backward_workspace_bytes(int32_t n_img, int32_t H, int32_t W, int32_t S, int32_t L, int32_t log2_T) {
     using namespace rf;
     if (n_img <= 0 || H <= 0 || W <= 0 || S < 1 || S > kMaxS || L < 1 || log2_T < 4 || log2_T > 24) return 0;
-    const long long n_tiles = (long long)n_img * sdb_div_up(H, kTileH) * sdb_div_up(W, kTileW);
-    return (int64_t)bwd_layout(n_tiles, S, L, log2_T).total;
+    return (int64_t)bwd_layout(view_tiles(H, W), S, L, log2_T).total;
 }
 
 // Diagnostics: byte offsets of the record (11 values: hdr, tile_list, tile_work, rayflags, x3, x0, act, mask, sig, nds, c) and of
@@ -374,9 +382,8 @@ extern "C" int sdb_debug_train_layout(int32_t n_img, int32_t H, int32_t W, int32
 {
     using namespace rf;
     if (!out || n_img <= 0 || H <= 0 || W <= 0 || S < 1 || S > kMaxS) return SDB_EINVAL;
-    const long long n_tiles = (long long)n_img * sdb_div_up(H, kTileH) * sdb_div_up(W, kTileW);
-    const RecordLayout r = record_layout(n_tiles, S);
-    const BwdLayout b = bwd_layout(n_tiles, S, L, log2_T);
+    const RecordLayout r = record_layout(n_img, n_img * view_tiles(H, W), S);
+    const BwdLayout b = bwd_layout(view_tiles(H, W), S, L, log2_T);
     const size_t v[20] = {r.hdr, r.tile_list, r.tile_work, r.rayflags, r.x3, r.x0, r.act, r.mask, r.sig, r.nds, r.c,
                           b.dc32, b.dc16, b.dsig32, b.dsig16, b.dz, b.dx0, b.dt3, r.total, b.total};
     for (int i = 0; i < 20; i++) out[i] = (int64_t)v[i];
@@ -394,19 +401,24 @@ extern "C" int sdb_render_rays_train_forward(const sdb_render_params *sp, void *
         if (rc != SDB_OK) return rc;
     }
     if (p.raw5d || sp->precision != 2) return SDB_EUNSUPPORTED;      // record + backward are built on the pre-blended table, fp16x3
-    if (p.n_img != 1) return SDB_EUNSUPPORTED;                        // one view (one style code) per record: the weight gradients are per style
+    if (p.n_img > 1 && (p.pack_stride < 0 || (p.pack_stride > 0 && p.pack_stride < packBytes<kRender>(2)))) return SDB_EINVAL;
     uint8_t *rec = (uint8_t *)d_record;
-    const RecordLayout rl = record_layout(p.n_tiles, p.S);
+    const RecordLayout rl = record_layout(p.n_img, p.n_tiles, p.S);
     bind_record(p, rec, rl);
     {
-        const int rc = launch_prepass(p, reinterpret_cast<int32_t *>(rec + rl.hdr), st);
+        const int rc = launch_train_prepass(p, reinterpret_cast<int32_t *>(rec + rl.hdr), reinterpret_cast<int32_t *>(rec + rl.tile_list), st);
         if (rc != SDB_OK) return rc;
     }
     const int grid = p.n_tiles < sdb_num_sms() ? p.n_tiles : sdb_num_sms();
     return launch_train_forward(p, grid, st);
 }
 
-extern "C" int sdb_render_rays_backward(const sdb_render_params *sp, const void *d_record, const sdb_render_grads *g, void *stream)
+// gradient strides between images, in floats: w1ext, wh, wsig, wout, sky_avg (one image's size each when n_img == 1)
+static const int64_t kRenderGradSize[5] = {(int64_t)rf::kHidden * rf::kX0Cols, (int64_t)5 * rf::kHidden * rf::kActCols,
+                                           (int64_t)8 * rf::kActCols, (int64_t)rf::kOutC * rf::kActCols, rf::kOutC};
+
+static int render_backward(const sdb_render_params *sp, const void *d_record, const sdb_render_grads *g, const int64_t *gstride,
+                           void *stream)
 {
     using namespace rf;
     if (!d_record || !g || !sp || !sp->d_cam_ori) return SDB_EINVAL;
@@ -419,11 +431,16 @@ extern "C" int sdb_render_rays_backward(const sdb_render_params *sp, const void 
         const int rc = params_from_abi(sp, p);
         if (rc != SDB_OK) return rc;
     }
-    if (p.raw5d || p.n_img != 1) return SDB_EUNSUPPORTED;
+    if (p.raw5d) return SDB_EUNSUPPORTED;
+    if (g->bwd_pack_stride < 0 || (p.n_img > 1 && g->bwd_pack_stride > 0 && g->bwd_pack_stride < packBytes<kBwd>(2))) return SDB_EINVAL;
+    for (int k = 0; k < 5; k++)
+        if (gstride[k] < 0 || (p.n_img > 1 && gstride[k] < kRenderGradSize[k])) return SDB_EINVAL;
     uint8_t *rec = (uint8_t *)const_cast<void *>(d_record);
-    const RecordLayout rl = record_layout(p.n_tiles, p.S);
+    const RecordLayout rl = record_layout(p.n_img, p.n_tiles, p.S);
     bind_record(p, rec, rl);
-    const BwdLayout bl = bwd_layout(p.n_tiles, p.S, sp->L, p.log2_T);
+    const int32_t *hdr = reinterpret_cast<const int32_t *>(rec + rl.hdr);
+    const long long tpi = p.n_tiles / p.n_img, hw = (long long)p.H * p.W;
+    const BwdLayout bl = bwd_layout(tpi, p.S, sp->L, p.log2_T);
     uint8_t *ws = (uint8_t *)g->d_workspace;
     float *dc32 = reinterpret_cast<float *>(ws + bl.dc32);
     uint16_t *dc16 = reinterpret_cast<uint16_t *>(ws + bl.dc16);
@@ -438,47 +455,90 @@ extern "C" int sdb_render_rays_backward(const sdb_render_params *sp, const void 
     const bool timing0 = getenv("SDB_TIMING") != nullptr;
     cudaEvent_t tev0 = nullptr;
     if (timing0) { cudaEventCreate(&tev0); cudaEventRecord(tev0, st); }
-    // The number of live ray tiles of the recorded pass stays ON THE DEVICE (record header): every kernel below is launched over
-    // the record's capacity and reads it there, so this call never synchronises -- the host can queue the whole backward (and the
-    // torch ops behind it) while the forward kernel is still running, which is what makes the step time independent of host speed.
-    const long long cap_items = (long long)p.n_tiles * p.S;
+    // The live-tile counts of the recorded pass stay ON THE DEVICE (record header): every kernel below is launched over one
+    // view's capacity and reads its image's {first, count} there, so this call never synchronises -- the host can queue the whole
+    // backward (and the torch ops behind it) while the forward kernel is still running, which is what makes the step time
+    // independent of host speed.
+    const long long cap_items = tpi * p.S;
     const size_t table_bytes = ((size_t)sp->L << p.log2_T) * 8 * 4;
 
-    SDB_CUDA(cudaMemsetAsync(g->d_grad_sky_avg, 0, (size_t)p.n_img * kOutC * 4, st));
+    for (int i = 0; i < p.n_img; i++)
+        SDB_CUDA(cudaMemsetAsync(g->d_grad_sky_avg + i * gstride[4], 0, (size_t)kOutC * 4, st));
     SDB_CUDA(cudaMemsetAsync(g->d_grad_global_enc, 0, 8, st));
     SDB_CUDA(cudaMemsetAsync(dt3, 0, table_bytes, st));
-
-    // SDB_TIMING=1: per-stage device times on stderr (diagnostics; synchronises)
-    const bool timing = getenv("SDB_TIMING") != nullptr;
-    cudaEvent_t tev[8];
-    int ntev = 0;
-    auto mark = [&]() { if (timing && ntev < 8) { cudaEventCreate(&tev[ntev]); cudaEventRecord(tev[ntev], st); ntev++; } };
-    mark();
-    // 1. compositing backward (every tile: sky-only tiles still feed dL/dsky)
-    composite_backward_kernel<<<p.n_tiles, 256, 0, st>>>(p, g->d_grad_net_out, g->d_grad_sky, g->d_grad_sky_avg, dc32, dc16,
-                                                         dsig32, dsig16);
-    SDB_CHECK_LAUNCH();
-    mark();
-    // 2. data-gradient chain on the tensor-core engine: one work item per (live tile, sample step) -- the slot index
-    //    (work * 1 + 0) * 128 + row of such an item IS the record's (tile * S + step) * 128 + row
-    {
-        Params pc = p;
-        pc.work_mult = p.S;
-        pc.S = 1;
-        const int grid = cap_items < sdb_num_sms() ? (int)cap_items : sdb_num_sms();      // work items beyond n_live * S do not exist: CTAs find none
-        const int rc = launch_bwd_chain(pc, grid, st);
-        if (rc != SDB_OK) return rc;
+    for (int i = 0; i < p.n_img; i++) {
+        SDB_CUDA(cudaMemsetAsync(g->d_grad_w1ext + i * gstride[0], 0, (size_t)kRenderGradSize[0] * 4, st));
+        SDB_CUDA(cudaMemsetAsync(g->d_grad_wh + i * gstride[1], 0, (size_t)kRenderGradSize[1] * 4, st));
+        SDB_CUDA(cudaMemsetAsync(g->d_grad_wsig + i * gstride[2], 0, (size_t)kRenderGradSize[2] * 4, st));
+        SDB_CUDA(cudaMemsetAsync(g->d_grad_wout + i * gstride[3], 0, (size_t)kRenderGradSize[3] * 4, st));
     }
+
+    // SDB_TIMING=1: per-stage device times on stderr, summed over the images (diagnostics; synchronises)
+    const bool timing = getenv("SDB_TIMING") != nullptr;
+    std::vector<cudaEvent_t> tev;
+    auto mark = [&]() { if (timing) { tev.emplace_back(); cudaEventCreate(&tev.back()); cudaEventRecord(tev.back(), st); } };
     mark();
-    // 3. table gradient: scatter into the pre-blended table, transpose of the pre-blend, scene code
+    for (int i = 0; i < p.n_img; i++) {
+        const int32_t *view = hdr + 1 + 2 * i;      // {first live-list position, live tiles} of image i
+        // 1. compositing backward over image i's tiles (every tile: sky-only tiles still feed dL/dsky)
+        {
+            Params pi = p;
+            pi.n_img = 1; pi.n_tiles = (int)tpi; pi.view = view;
+            pi.cam_ori = p.cam_ori + 3 * i;
+            pi.sky = p.sky + i * hw * kOutC; pi.sky_avg = p.sky_avg + i * kOutC;
+            pi.tr.tile_work = p.tr.tile_work + i * tpi;
+            composite_backward_kernel<<<(unsigned)tpi, 256, 0, st>>>(pi, g->d_grad_net_out + i * hw * kOutC, g->d_grad_sky + i * hw * kOutC,
+                                                                     g->d_grad_sky_avg + i * gstride[4], dc32, dc16, dsig32, dsig16);
+            SDB_CHECK_LAUNCH();
+        }
+        mark();
+        // 2. data-gradient chain on the tensor-core engine: one work item per (live tile, sample step) of image i -- the slot
+        //    index (work * 1 + 0) * 128 + row of such an item IS the workspace's (tile * S + step) * 128 + row
+        Params pv = p;
+        pv.view = view;
+        pv.n_live = view + 1;
+        {
+            Params pc = pv;
+            pc.work_mult = p.S;
+            pc.S = 1;
+            pc.tr.slot_cap = cap_items * kRows;      // layer stride of dZ in the (one-view) workspace
+            const int grid = cap_items < sdb_num_sms() ? (int)cap_items : sdb_num_sms();      // items beyond count * S do not exist: CTAs find none
+            const int rc = launch_bwd_chain(pc, grid, st);
+            if (rc != SDB_OK) return rc;
+        }
+        mark();
+        // 3a. scatter image i's feature gradients into the pre-blended table gradient (shared by all images)
+        {
+            dim3 grid((unsigned)((cap_items * kRows + 255) / 256), kLevels);
+            // SDB_TABLE_AGG_LEVELS: tuning knob (levels 0..n-1 use the warp-aggregated scatter); the default was chosen on the
+            // previous GPU generation and is carried over, not re-measured on H100
+            int agg_levels = 12;
+            if (const char *e = getenv("SDB_TABLE_AGG_LEVELS")) agg_levels = atoi(e);
+            table3_backward_kernel<<<grid, 256, 0, st>>>(pv, dx0, dt3, agg_levels);
+            SDB_CHECK_LAUNCH();
+        }
+        mark();
+        // 4. image i's weight gradients on the tensor cores (its live items, nothing else: no padding rows to zero).
+        //    A = the record (the image's items start at view[0] * S), Z = the workspace.
+        {
+            const long long cap = p.tr.slot_cap, wcap = cap_items * kRows;
+            float *w1ext = g->d_grad_w1ext + i * gstride[0], *wh = g->d_grad_wh + i * gstride[1];
+            float *wsig = g->d_grad_wsig + i * gstride[2], *wout = g->d_grad_wout + i * gstride[3];
+            WgJob jobs[kWgMaxJobs];
+            int nj = 0;
+            add_jobs(jobs, nj, p.tr.x0, kX0Cols, dz, kHidden, w1ext, kHidden);                                             // fc_1 | fc_m_a | bias
+            for (int k = 0; k < 5; k++)                                                                                    // fc_2 .. fc_6
+                add_jobs(jobs, nj, p.tr.act + (size_t)k * cap * kActCols, kActCols, dz + (size_t)(k + 1) * wcap * kHidden, kHidden,
+                         wh + (size_t)k * kHidden * kActCols, kHidden);
+            add_jobs(jobs, nj, p.tr.act + (size_t)5 * cap * kActCols, kActCols, dc16, kOutC, wout, kOutC);                // fc_out_c
+            add_jobs(jobs, nj, p.tr.act + (size_t)3 * cap * kActCols, kActCols, dsig16, 8, wsig, 8);                      // fc_sigma
+            const int rc = launch_wgrad(jobs, nj, view, p.S, cap_items, st);
+            if (rc != SDB_OK) return rc;
+        }
+        mark();
+    }
+    // 3b. table gradient of the batch: transpose of the pre-blend, scene code (once for all images)
     {
-        dim3 grid((unsigned)((cap_items * kRows + 255) / 256), kLevels);
-        // SDB_TABLE_AGG_LEVELS: tuning knob (levels 0..n-1 use the warp-aggregated scatter); the default was chosen on the
-        // previous GPU generation and is carried over, not re-measured on H100
-        int agg_levels = 12;
-        if (const char *e = getenv("SDB_TABLE_AGG_LEVELS")) agg_levels = atoi(e);
-        table3_backward_kernel<<<grid, 256, 0, st>>>(p, dx0, dt3, agg_levels);
-        SDB_CHECK_LAUNCH();
         int rc = sdb_preblend_table(dt3, g->d_grad_table, sp->L, p.log2_T, p.level_S, p.base_res, p.genc, stream);
         if (rc != SDB_OK) return rc;
         const size_t n = (size_t)sp->L << p.log2_T;
@@ -487,87 +547,114 @@ extern "C" int sdb_render_rays_backward(const sdb_render_params *sp, const void 
         SDB_CHECK_LAUNCH();
     }
     mark();
-    // 4. weight gradients on the tensor cores (every live item, nothing else: no padding rows to zero)
-    {
-        SDB_CUDA(cudaMemsetAsync(g->d_grad_w1ext, 0, (size_t)kHidden * kX0Cols * 4, st));
-        SDB_CUDA(cudaMemsetAsync(g->d_grad_wh, 0, (size_t)5 * kHidden * kActCols * 4, st));
-        SDB_CUDA(cudaMemsetAsync(g->d_grad_wsig, 0, (size_t)8 * kActCols * 4, st));
-        SDB_CUDA(cudaMemsetAsync(g->d_grad_wout, 0, (size_t)kOutC * kActCols * 4, st));
-        const long long cap = p.tr.slot_cap;
-        WgJob jobs[kWgMaxJobs];
-        int nj = 0;
-        add_jobs(jobs, nj, p.tr.x0, kX0Cols, dz, kHidden, g->d_grad_w1ext, kHidden);                                  // fc_1 | fc_m_a | bias
-        for (int k = 0; k < 5; k++)                                                                                    // fc_2 .. fc_6
-            add_jobs(jobs, nj, p.tr.act + (size_t)k * cap * kActCols, kActCols, dz + (size_t)(k + 1) * cap * kHidden, kHidden,
-                     g->d_grad_wh + (size_t)k * kHidden * kActCols, kHidden);
-        add_jobs(jobs, nj, p.tr.act + (size_t)5 * cap * kActCols, kActCols, dc16, kOutC, g->d_grad_wout, kOutC);       // fc_out_c
-        add_jobs(jobs, nj, p.tr.act + (size_t)3 * cap * kActCols, kActCols, dsig16, 8, g->d_grad_wsig, 8);             // fc_sigma
-        const int rc = launch_wgrad(jobs, nj, p.n_live, p.S, cap_items, st);
-        if (rc != SDB_OK) return rc;
-    }
-    mark();
     if (timing) {
         cudaStreamSynchronize(st);
-        float ms[8] = {0};
-        for (int i = 0; i + 1 < ntev; i++) cudaEventElapsedTime(&ms[i], tev[i], tev[i + 1]);
+        float ms[4] = {0, 0, 0, 0}, untable = 0.0f;
+        for (int i = 0; i < p.n_img; i++)
+            for (int k = 0; k < 4; k++) {
+                float t = 0.0f;
+                cudaEventElapsedTime(&t, tev[4 * i + k], tev[4 * i + k + 1]);
+                ms[k] += t;
+            }
+        cudaEventElapsedTime(&untable, tev[4 * p.n_img], tev[4 * p.n_img + 1]);
         float pre = 0.0f;
         if (tev0) { cudaEventElapsedTime(&pre, tev0, tev[0]); cudaEventDestroy(tev0); }
         int32_t n_live = 0;
         cudaMemcpy(&n_live, rec + rl.hdr, 4, cudaMemcpyDeviceToHost);
         fprintf(stderr, "[sdb timing] backward: prologue %.3f ms, compositing %.3f ms, chain %.3f ms, table %.3f ms, weight GEMMs %.3f ms (n_live %d)\n",
-                pre, ms[0], ms[1], ms[2], ms[3], n_live);
-        for (int i = 0; i < ntev; i++) cudaEventDestroy(tev[i]);
+                pre, ms[0], ms[1], ms[2] + untable, ms[3], n_live);
+        for (cudaEvent_t e : tev) cudaEventDestroy(e);
     }
     return SDB_OK;
 }
 
+extern "C" int sdb_render_rays_backward(const sdb_render_params *sp, const void *d_record, const sdb_render_grads *g, void *stream)
+{
+    if (sp && sp->n_img != 1) return sp->n_img < 1 ? SDB_EINVAL : SDB_EUNSUPPORTED;      // one set of weight gradients: see _views
+    return render_backward(sp, d_record, g, kRenderGradSize, stream);
+}
+
+extern "C" int sdb_render_rays_backward_views(const sdb_render_params *sp, const void *d_record, const sdb_render_view_grads *vg,
+                                              void *stream)
+{
+    if (!vg) return SDB_EINVAL;
+    const int64_t stride[5] = {vg->w1ext_stride, vg->wh_stride, vg->wsig_stride, vg->wout_stride, vg->sky_avg_stride};
+    return render_backward(sp, d_record, &vg->g, stride, stream);
+}
+
 // ---- sky branch (a9) backward: SKYMLP data-gradient chain on the tensor-core engine + weight-gradient GEMMs -------------
-// (gancraft_base.py:150-169 under autograd; the positional encoding of the ray direction needs no gradient)
+// (gancraft_base.py:150-169 under autograd; the positional encoding of the ray direction needs no gradient).  Image by image
+// over one view-sized workspace, like the render backward.
 extern "C" int64_t sdb_sky_backward_workspace_bytes(int32_t n_img, int32_t H, int32_t W) {
     using namespace rf;
     if (n_img <= 0 || H <= 0 || W <= 0) return 0;
-    return (int64_t)sky_bwd_layout((long long)n_img * sdb_div_up(H, kTileH) * sdb_div_up(W, kTileW)).total;
+    return (int64_t)sky_bwd_layout(view_tiles(H, W)).total;
+}
+
+static const int64_t kSkyGradSize[3] = {(int64_t)rf::kHidden * rf::kSkyK0, (int64_t)4 * rf::kHidden * rf::kActCols,
+                                        (int64_t)rf::kOutC * rf::kActCols};
+
+extern "C" int sdb_sky_backward_views(int32_t n_img, int32_t H, int32_t W, const void *d_record, const float *d_grad_sky,
+                                      const void *d_bwd_pack, int64_t bwd_pack_stride, const sdb_sky_view_grads *g,
+                                      void *d_workspace, void *stream)
+{
+    using namespace rf;
+    if (!d_record || !d_grad_sky || !d_bwd_pack || !g || !g->d_grad_w1ext || !g->d_grad_wh || !g->d_grad_wout || !d_workspace)
+        return SDB_EINVAL;
+    if (n_img <= 0 || H <= 0 || W <= 0) return SDB_EINVAL;
+    const int64_t gstride[3] = {g->w1ext_stride, g->wh_stride, g->wout_stride};
+    if (bwd_pack_stride < 0 || (n_img > 1 && bwd_pack_stride > 0 && bwd_pack_stride < packBytes<kSkyBwd>(2))) return SDB_EINVAL;
+    for (int k = 0; k < 3; k++)
+        if (gstride[k] < 0 || (n_img > 1 && gstride[k] < kSkyGradSize[k])) return SDB_EINVAL;
+    cudaStream_t st = (cudaStream_t)stream;
+    const long long tpi = view_tiles(H, W), hw = (long long)H * W;
+    const long long cap = n_img * tpi * kRows, vcap = tpi * kRows;      // slots of the record / of one view
+    const SkyRecordLayout rl = sky_record_layout(n_img * tpi);
+    const SkyBwdLayout bl = sky_bwd_layout(tpi);
+    uint8_t *rec = (uint8_t *)const_cast<void *>(d_record), *ws = (uint8_t *)d_workspace;
+    for (int i = 0; i < n_img; i++) {
+        // image i: its tiles (slot = tile * 128 + row over the frame) are record slots [i * vcap, (i + 1) * vcap)
+        Params p{};
+        p.n_img = 1; p.H = H; p.W = W; p.M = 1; p.S = 1;
+        p.tiles_x = sdb_div_up(W, kTileW); p.tiles_y = sdb_div_up(H, kTileH);
+        p.n_tiles = (int)tpi;
+        p.pack = (const uint8_t *)d_bwd_pack + i * bwd_pack_stride; p.pack_stride = 0;
+        p.debug = g_debug_buffer;
+        p.tr.slot_cap = vcap;
+        p.tr.mask = reinterpret_cast<uint32_t *>(rec + rl.mask) + (size_t)i * tpi * kNumAct * kRows * 8;
+        p.tr.dc = d_grad_sky + i * hw * kOutC;
+        p.tr.dc16 = reinterpret_cast<uint16_t *>(ws + bl.dc16);
+        p.tr.dz = reinterpret_cast<uint16_t *>(ws + bl.dz);
+        {
+            const int grid = p.n_tiles < sdb_num_sms() ? p.n_tiles : sdb_num_sms();
+            const int rc = launch_sky_bwd_chain(p, grid, st);
+            if (rc != SDB_OK) return rc;
+        }
+        float *w1ext = g->d_grad_w1ext + i * gstride[0], *wh = g->d_grad_wh + i * gstride[1], *wout = g->d_grad_wout + i * gstride[2];
+        SDB_CUDA(cudaMemsetAsync(w1ext, 0, (size_t)kSkyGradSize[0] * 4, st));
+        SDB_CUDA(cudaMemsetAsync(wh, 0, (size_t)kSkyGradSize[1] * 4, st));
+        SDB_CUDA(cudaMemsetAsync(wout, 0, (size_t)kSkyGradSize[2] * 4, st));
+        const uint16_t *x0 = reinterpret_cast<const uint16_t *>(rec + rl.x0) + (size_t)i * vcap * kSkyK0;
+        const uint16_t *act = reinterpret_cast<const uint16_t *>(rec + rl.act) + (size_t)i * vcap * kActCols;
+        WgJob jobs[kWgMaxJobs];
+        int nj = 0;
+        add_jobs(jobs, nj, x0, kSkyK0, p.tr.dz, kHidden, w1ext, kHidden);                                                  // fc1 | bias
+        for (int k = 0; k < 4; k++)                                                                                        // fc2 .. fc5
+            add_jobs(jobs, nj, act + (size_t)k * cap * kActCols, kActCols, p.tr.dz + (size_t)(k + 1) * vcap * kHidden, kHidden,
+                     wh + (size_t)k * kHidden * kActCols, kHidden);
+        add_jobs(jobs, nj, act + (size_t)4 * cap * kActCols, kActCols, p.tr.dc16, kOutC, wout, kOutC);                     // fc_out_c
+        const int rc = launch_wgrad(jobs, nj, nullptr, 1, tpi, st);
+        if (rc != SDB_OK) return rc;
+    }
+    return SDB_OK;
 }
 
 extern "C" int sdb_sky_backward(int32_t n_img, int32_t H, int32_t W, const void *d_record, const float *d_grad_sky,
                                 const void *d_bwd_pack, float *d_grad_w1ext, float *d_grad_wh, float *d_grad_wout,
                                 void *d_workspace, void *stream)
 {
-    using namespace rf;
     if (!d_record || !d_grad_sky || !d_bwd_pack || !d_grad_w1ext || !d_grad_wh || !d_grad_wout || !d_workspace) return SDB_EINVAL;
     if (n_img != 1 || H <= 0 || W <= 0) return n_img == 1 ? SDB_EINVAL : SDB_EUNSUPPORTED;
-    cudaStream_t st = (cudaStream_t)stream;
-    Params p{};
-    p.n_img = n_img; p.H = H; p.W = W; p.M = 1; p.S = 1;
-    p.tiles_x = sdb_div_up(W, kTileW); p.tiles_y = sdb_div_up(H, kTileH);
-    p.n_tiles = n_img * p.tiles_x * p.tiles_y;
-    p.pack = (const uint8_t *)d_bwd_pack; p.pack_stride = 0;
-    p.debug = g_debug_buffer;
-    const SkyRecordLayout rl = sky_record_layout(p.n_tiles);
-    const SkyBwdLayout bl = sky_bwd_layout(p.n_tiles);
-    uint8_t *rec = (uint8_t *)const_cast<void *>(d_record), *ws = (uint8_t *)d_workspace;
-    const long long cap = (long long)p.n_tiles * kRows;
-    p.tr.slot_cap = cap;
-    p.tr.x0 = reinterpret_cast<uint16_t *>(rec + rl.x0);
-    p.tr.act = reinterpret_cast<uint16_t *>(rec + rl.act);
-    p.tr.mask = reinterpret_cast<uint32_t *>(rec + rl.mask);
-    p.tr.dc = d_grad_sky;
-    p.tr.dc16 = reinterpret_cast<uint16_t *>(ws + bl.dc16);
-    p.tr.dz = reinterpret_cast<uint16_t *>(ws + bl.dz);
-    {
-        const int grid = p.n_tiles < sdb_num_sms() ? p.n_tiles : sdb_num_sms();
-        const int rc = launch_sky_bwd_chain(p, grid, st);
-        if (rc != SDB_OK) return rc;
-    }
-    SDB_CUDA(cudaMemsetAsync(d_grad_w1ext, 0, (size_t)kHidden * kSkyK0 * 4, st));
-    SDB_CUDA(cudaMemsetAsync(d_grad_wh, 0, (size_t)4 * kHidden * kActCols * 4, st));
-    SDB_CUDA(cudaMemsetAsync(d_grad_wout, 0, (size_t)kOutC * kActCols * 4, st));
-    WgJob jobs[kWgMaxJobs];
-    int nj = 0;
-    add_jobs(jobs, nj, p.tr.x0, kSkyK0, p.tr.dz, kHidden, d_grad_w1ext, kHidden);                                              // fc1 | bias
-    for (int k = 0; k < 4; k++)                                                                                               // fc2 .. fc5
-        add_jobs(jobs, nj, p.tr.act + (size_t)k * cap * kActCols, kActCols, p.tr.dz + (size_t)(k + 1) * cap * kHidden, kHidden,
-                 d_grad_wh + (size_t)k * kHidden * kActCols, kHidden);
-    add_jobs(jobs, nj, p.tr.act + (size_t)4 * cap * kActCols, kActCols, p.tr.dc16, kOutC, d_grad_wout, kOutC);                // fc_out_c
-    return launch_wgrad(jobs, nj, nullptr, 1, p.n_tiles, st);
+    const sdb_sky_view_grads g{d_grad_w1ext, 0, d_grad_wh, 0, d_grad_wout, 0};
+    return sdb_sky_backward_views(n_img, H, W, d_record, d_grad_sky, d_bwd_pack, 0, &g, d_workspace, stream);
 }

@@ -183,6 +183,7 @@ struct Params {
     int32_t *debug;                // optional host-mapped progress buffer (diagnostics), else nullptr
     TrainBuf tr;                   // training record (TRAIN forward writes it, the kBwd chain reads it)
     float *acc;                    // [grid][2][128][256] fp32 accumulator buffers, set by the launcher
+    const int32_t *view;           // kBwd over one image of a multi-view record: {first live-list position, live tiles} (device)
 };
 
 // NV consecutive fp32 accumulators of one row (written by the MMA warpgroup of the same CTA: plain loads, not the
@@ -330,6 +331,7 @@ int launch_bwd_chain(const Params &p, int grid, cudaStream_t st);         // mlp
 int launch_sky_train_forward(const Params &p, int grid, cudaStream_t st); // mlp_kernel<fp16x3, -, kSky, TRAIN>
 int launch_sky_bwd_chain(const Params &p, int grid, cudaStream_t st);     // mlp_kernel<bf16x3, -, kSkyBwd>
 int launch_prepass(const Params &p, int32_t *ws, cudaStream_t st);        // zeroes the counter, fills tile list (+ tile_work)
+int launch_train_prepass(const Params &p, int32_t *hdr, int32_t *tile_list, cudaStream_t st);   // live tiles grouped by image
 int params_from_abi(const sdb_render_params *sp, Params &p);        // validate + translate the ABI struct
 extern int32_t *g_debug_buffer;
 

@@ -32,7 +32,7 @@ constexpr uint32_t kWgSmem = kWgStages * kWgStageBytes + 256;
 struct WgParams {
     WgJob job[kWgMaxJobs];
     int n_jobs;
-    const int32_t *n_live;       // device: live ray tiles of the recorded pass (nullptr: every item up to cap_items exists)
+    const int32_t *view;         // device: {first, count} live ray tiles of the recorded pass (nullptr: every item up to cap_items exists)
     int items_per_live;
     long long cap_items;
 };
@@ -48,8 +48,9 @@ wgrad_kernel(const WgParams prm)
     int j = 0, split = blockIdx.x;
     while (j < prm.n_jobs && split >= prm.job[j].nsplit) { split -= prm.job[j].nsplit; j++; }
     if (j >= prm.n_jobs) return;
-    const WgJob jb = prm.job[j];
-    const long long n_items = prm.n_live ? (long long)__ldg(prm.n_live) * prm.items_per_live : prm.cap_items;
+    WgJob jb = prm.job[j];
+    const long long n_items = prm.view ? (long long)__ldg(prm.view + 1) * prm.items_per_live : prm.cap_items;
+    if (prm.view) jb.A += (size_t)__ldg(prm.view) * prm.items_per_live * jb.a_chunks * (kChunkBytes / 2);      // A: this image's record items
     const long long my_items = split < n_items ? (n_items - split + jb.nsplit - 1) / jb.nsplit : 0;
 
     // dZ chunks the job does not own stay zero for the whole kernel (M-tiles narrower than 128 rows: fc_out_c, fc_sigma)
@@ -124,14 +125,14 @@ wgrad_kernel(const WgParams prm)
 }  // namespace
 
 // Splits: CTAs are handed out in proportion to the bytes a job streams per item, one CTA per SM over the whole list.
-int launch_wgrad(WgJob *jobs, int n_jobs, const int32_t *d_n_live, int items_per_live, long long cap_items, cudaStream_t st)
+int launch_wgrad(WgJob *jobs, int n_jobs, const int32_t *d_view, int items_per_live, long long cap_items, cudaStream_t st)
 {
     if (n_jobs < 1 || n_jobs > kWgMaxJobs) return SDB_EINVAL;
     if (cap_items <= 0) return SDB_OK;
     const long long n_items = cap_items;
     WgParams prm{};
     prm.n_jobs = n_jobs;
-    prm.n_live = d_n_live;
+    prm.view = d_view;
     prm.items_per_live = items_per_live;
     prm.cap_items = cap_items;
     double total = 0.0;

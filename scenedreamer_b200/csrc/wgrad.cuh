@@ -20,9 +20,10 @@ struct WgJob {
     int nsplit;
 };
 
-// dW += over the first n_items work items (128 samples each); `out` buffers must have been zeroed on the stream.
-// n_items = *d_n_live * items_per_live read ON THE DEVICE (no host round trip), or cap_items when d_n_live is null;
-// cap_items (the record's capacity) only sizes the split of the jobs over the CTAs.
-int launch_wgrad(WgJob *jobs, int n_jobs, const int32_t *d_n_live, int items_per_live, long long cap_items, cudaStream_t st);
+// dW += over n_items work items (128 samples each); `out` buffers must have been zeroed on the stream.
+// d_view = {first, count} in live tiles, read ON THE DEVICE (no host round trip): n_items = count * items_per_live, and the
+// items of A start at first * items_per_live (Z holds only these items); d_view null: every item up to cap_items, no offset.
+// cap_items (the capacity of one view) only sizes the split of the jobs over the CTAs.
+int launch_wgrad(WgJob *jobs, int n_jobs, const int32_t *d_view, int items_per_live, long long cap_items, cudaStream_t st);
 
 }  // namespace rf

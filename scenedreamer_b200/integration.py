@@ -47,6 +47,13 @@ def enabled():
     return os.environ.get('SDB200_FUSED', '1') not in ('0', 'false', 'False', 'off')
 
 
+def train_views_enabled():
+    """SDB200_TRAIN_VIEWS=1: a batch under autograd is one recorded training pass (render.render_rays_train over all its
+    views), and a preset self.sky_avg is every view's sky mean on that pass.  Off by default: one pass per view, and a
+    preset sky_avg defers to the reference's composition, as before the batched pass existed."""
+    return os.environ.get('SDB200_TRAIN_VIEWS', '0') not in ('0', 'false', 'False', 'off', '')
+
+
 # ------------------------------------------------------------------------------------------------
 # per-instance state
 # ------------------------------------------------------------------------------------------------
@@ -255,10 +262,12 @@ def fused_forward_perpix(self, blk_feats, voxel_id, depth2, raydirs, cam_ori_t, 
         return reference(self, blk_feats, voxel_id, depth2, raydirs, cam_ori_t, z, global_enc)
     needs_grad = _needs_grad(self, z, global_enc)
     N, H, W = voxel_id.shape[:3]
+    train_views = train_views_enabled()
     if needs_grad:
-        # differentiating through a caller-supplied sky_avg or through views of different scenes is left to the reference
+        # differentiating through views of different scenes is left to the reference (the pre-blended table is per scene), and
+        # so is a caller-supplied sky_avg unless the batched training pass is switched on
         one_scene = global_enc.shape[0] == 1 or bool((global_enc == global_enc[:1]).all())
-        if hasattr(self, 'sky_avg') or not one_scene:
+        if not one_scene or (hasattr(self, 'sky_avg') and not train_views):
             st.stats['reference_calls'] += 1
             return reference(self, blk_feats, voxel_id, depth2, raydirs, cam_ori_t, z, global_enc)
     uniforms = None
@@ -268,19 +277,25 @@ def fused_forward_perpix(self, blk_feats, voxel_id, depth2, raydirs, cam_ori_t, 
     sky_only_mask = voxel_id[:, :, :, [0], :] == 0
     kw = dict(num_samples=self.num_samples, sample_depth=self.sample_depth, dists_scale=self.dists_scale)
     if needs_grad:
-        # one recorded pass per view (one style code each); the frame mean of the sky features is per view as well
-        # (scenedreamer.py:395 averages over dims 1,2 only), so a batch is exactly the concatenation of its views
+        # SDB200_TRAIN_VIEWS=1: the views of the batch in ONE recorded pass, each with its own style code, camera and sky mean
+        # (the frame mean of its sky features, scenedreamer.py:395 averages over dims 1,2 only; or the preset self.sky_avg,
+        # :391-392, which inference_givenstyle leaves behind).  Otherwise one recorded pass per view.
         st.stats['train_calls'] += 1
         he = self.hash_encoder
         P = _live_params(self)
-        outs = []
-        for i in range(N):
-            outs.append(render.render_rays_train(
+        sky_attr = getattr(self, 'sky_avg', None)
+        sky_avg = None if sky_attr is None else sky_attr.reshape(-1, 64).expand(N, 64)
+        args = ([float(v) for v in self.voxel.voxel_t.shape], st.lut, he.per_level_scale)
+        kw.update(base_res=he.base_resolution, log2_T=he.log2_hashmap_size, L=he.num_levels)
+        if train_views:
+            out = render.render_rays_train(P, voxel_id.contiguous(), depth2.contiguous(), raydirs.contiguous(), cam_ori_t, z,
+                                           global_enc[:1], *args, uniforms=uniforms, sky_avg=sky_avg, **kw)
+        else:
+            outs = [render.render_rays_train(
                 P, voxel_id[i:i + 1].contiguous(), depth2[i:i + 1].contiguous(), raydirs[i:i + 1].contiguous(),
-                cam_ori_t[i:i + 1], z[i:i + 1], global_enc[:1], [float(v) for v in self.voxel.voxel_t.shape], st.lut,
-                he.per_level_scale, uniforms=None if uniforms is None else uniforms[i:i + 1],
-                base_res=he.base_resolution, log2_T=he.log2_hashmap_size, L=he.num_levels, **kw))
-        out = {k: torch.cat([o[k] for o in outs], 0) for k in ('net_out', 'total_weight', 'weights', 'rand_depth', 'sky')}
+                cam_ori_t[i:i + 1], z[i:i + 1], global_enc[:1], *args, uniforms=None if uniforms is None else uniforms[i:i + 1],
+                sky_avg=None if sky_avg is None else sky_avg[i:i + 1], **kw) for i in range(N)]
+            out = {k: torch.cat([o[k] for o in outs], 0) for k in ('net_out', 'total_weight', 'weights', 'rand_depth', 'sky')}
         return _tuple12(out, sky_mask, sky_only_mask)
     st.stats['fused_calls'] += 1
     r = st.get_renderer(self)

@@ -412,6 +412,21 @@ class _RenderGrads(ctypes.Structure):
     ]
 
 
+class _RenderViewGrads(ctypes.Structure):
+    _fields_ = [('g', _RenderGrads), ('w1ext_stride', ctypes.c_int64), ('wh_stride', ctypes.c_int64),
+                ('wsig_stride', ctypes.c_int64), ('wout_stride', ctypes.c_int64), ('sky_avg_stride', ctypes.c_int64)]
+
+
+class _SkyViewGrads(ctypes.Structure):
+    _fields_ = [('d_grad_w1ext', ctypes.c_void_p), ('w1ext_stride', ctypes.c_int64), ('d_grad_wh', ctypes.c_void_p),
+                ('wh_stride', ctypes.c_int64), ('d_grad_wout', ctypes.c_void_p), ('wout_stride', ctypes.c_int64)]
+
+
+def _view_sum(g):
+    """Gradient of a tensor all views share: the sum of the per-view gradients [N, ...] (the one view itself when N == 1)."""
+    return g[0] if g.shape[0] == 1 else g.sum(0)
+
+
 def _fill_render_params(prm, keep, voxel_id, depth2, raydirs, cam_ori, genc, voxel_dims, lut, mlp_pack, sky, sky_avg, *,
                         table=None, table3=None, S, sample_depth, dists_scale, uniforms, precision, per_level_scale, base_res,
                         log2_T, L, net_out, depth, tw, wts, rdp, ws, early_stop=0.0):
@@ -454,9 +469,10 @@ def _fill_render_params(prm, keep, voxel_id, depth2, raydirs, cam_ori, genc, vox
 class _FusedRenderTrainFn(torch.autograd.Function):
     """net_out = fused_render(embeddings, global_enc, effective LightningMLP weights, sky, sky_avg).
 
-    The effective weights are what ModLinear produces for ONE style code (W' = W * alpha, beta; layers.py:247-260):
-    the caller computes them with ordinary torch ops so that autograd carries dL/dW', dL/dbeta on to the raw
-    parameters and to the style code.  One view per call (the training configs use batch 1 per GPU)."""
+    N views of one scene in one recorded pass.  wh [N,5,256,256], bh [N,5,256] are what ModLinear produces for each
+    view's style code (W' = W * alpha, beta; layers.py:247-260): the caller computes them with ordinary torch ops so that
+    autograd carries dL/dW', dL/dbeta on to the raw parameters and to the style codes.  sky [N,H,W,64], sky_avg [N,64];
+    genc holds the one scene code of all views.  The weights every view shares get the sum of the per-view gradients."""
 
     @staticmethod
     def forward(ctx, cfg, embeddings, genc, w1, b1, fc_m_a, wh, bh, wsig, bsig, wout, bout, sky, sky_avg):
@@ -464,8 +480,8 @@ class _FusedRenderTrainFn(torch.autograd.Function):
         voxel_id, depth2, raydirs = cfg['voxel_id'], cfg['depth2'], cfg['raydirs']
         dev = voxel_id.device
         N, H, W, M = voxel_id.shape[:4]
-        if N != 1:
-            raise RuntimeError('fused training path renders one view per call')
+        if tuple(wh.shape[:2]) != (N, 5) or tuple(bh.shape[:2]) != (N, 5):
+            raise RuntimeError('fused training path: wh / bh need one [5, ...] set per view')
         S = int(cfg['num_samples'])
         for t, n in ((voxel_id, 'voxel_id'), (depth2, 'depth2'), (raydirs, 'raydirs')):
             if not t.is_cuda or not t.is_contiguous():
@@ -480,9 +496,11 @@ class _FusedRenderTrainFn(torch.autograd.Function):
         lut = cfg['lut'].to(dev, torch.int32).contiguous()
         prec = PRECISION_FP16X3
         with torch.cuda.device(dev):
-            pack = torch.empty(int(L.sdb_mlp_pack_bytes(prec)), dtype=torch.uint8, device=dev)
-            _lib.check(L.sdb_pack_mlp(_ptr(w1_), _ptr(b1_), _ptr(emb_), int(emb_.shape[0]), _ptr(wh_), _ptr(bh_), _ptr(wsig_),
-                                      _ptr(bsig_), _ptr(wout_), _ptr(bout_), prec, _ptr(pack), _stream(dev)), 'sdb_pack_mlp')
+            pack = torch.empty(N, int(L.sdb_mlp_pack_bytes(prec)), dtype=torch.uint8, device=dev)      # one pack per view
+            for i in range(N):
+                _lib.check(L.sdb_pack_mlp(_ptr(w1_), _ptr(b1_), _ptr(emb_), int(emb_.shape[0]), _ptr(wh_[i]), _ptr(bh_[i]),
+                                          _ptr(wsig_), _ptr(bsig_), _ptr(wout_), _ptr(bout_), prec, _ptr(pack[i]), _stream(dev)),
+                           'sdb_pack_mlp')
             table3 = preblend_table(embeddings_, genc_, cfg['log2_T'], cfg['per_level_scale'], cfg['base_res'], cfg['L'])
             net_out = torch.empty(N, H, W, 64, dtype=torch.float32, device=dev)
             depth = torch.empty(N, H, W, dtype=torch.float32, device=dev)
@@ -504,7 +522,7 @@ class _FusedRenderTrainFn(torch.autograd.Function):
         ctx.record = record
         ctx.saved = (embeddings_, w1_, wh_, wsig_, wout_)
         ctx.shapes = (tuple(fc_m_a.shape), tuple(wsig.shape), tuple(bsig.shape), tuple(sky.shape), tuple(sky_avg.shape),
-                      tuple(genc.shape))
+                      tuple(genc.shape), tuple(wh.shape), tuple(bh.shape))
         ctx.mark_non_differentiable(depth, tw, wts, rdp)
         return net_out, depth, tw, wts, rdp
 
@@ -520,66 +538,73 @@ class _FusedRenderTrainFn(torch.autograd.Function):
         N, H, W, S = prm.n_img, prm.H, prm.W, prm.S
         g = g_net_out.to(torch.float32).contiguous()
         with torch.cuda.device(dev):
-            bpack = torch.empty(int(L.sdb_mlp_backward_pack_bytes()), dtype=torch.uint8, device=dev)
-            _lib.check(L.sdb_pack_mlp_backward(_ptr(w1_), _ptr(wh_), _ptr(wsig_), _ptr(wout_), _ptr(bpack), _stream(dev)),
-                       'sdb_pack_mlp_backward')
+            bpack = torch.empty(N, int(L.sdb_mlp_backward_pack_bytes()), dtype=torch.uint8, device=dev)      # one per view
+            for i in range(N):
+                _lib.check(L.sdb_pack_mlp_backward(_ptr(w1_), _ptr(wh_[i]), _ptr(wsig_), _ptr(wout_), _ptr(bpack[i]), _stream(dev)),
+                           'sdb_pack_mlp_backward')
             g_table = torch.empty_like(embeddings_)
             g_genc = torch.empty(2, dtype=torch.float32, device=dev)
-            g_w1ext = torch.empty(256, 144, dtype=torch.float32, device=dev)
-            g_wh = torch.empty(5, 256, 272, dtype=torch.float32, device=dev)
-            g_wsig = torch.empty(8, 272, dtype=torch.float32, device=dev)
-            g_wout = torch.empty(64, 272, dtype=torch.float32, device=dev)
+            g_w1ext = torch.empty(N, 256, 144, dtype=torch.float32, device=dev)
+            g_wh = torch.empty(N, 5, 256, 272, dtype=torch.float32, device=dev)
+            g_wsig = torch.empty(N, 8, 272, dtype=torch.float32, device=dev)
+            g_wout = torch.empty(N, 64, 272, dtype=torch.float32, device=dev)
             g_sky = torch.zeros(N, H, W, 64, dtype=torch.float32, device=dev)
             g_sky_avg = torch.empty(N, 64, dtype=torch.float32, device=dev)
             wsb = _take_scratch(L.sdb_render_backward_workspace_bytes(N, H, W, S, int(cfg['L']), int(cfg['log2_T'])), dev, 'bwd')
-            gr = _RenderGrads()
-            gr.d_grad_net_out, gr.d_bwd_pack, gr.bwd_pack_stride = _ptr(g), _ptr(bpack), 0
+            vg = _RenderViewGrads()
+            gr = vg.g
+            gr.d_grad_net_out, gr.d_bwd_pack, gr.bwd_pack_stride = _ptr(g), _ptr(bpack), int(bpack.stride(0))
             gr.d_table = _ptr(embeddings_)
             gr.d_grad_table, gr.d_grad_global_enc, gr.d_grad_w1ext = _ptr(g_table), _ptr(g_genc), _ptr(g_w1ext)
             gr.d_grad_wh, gr.d_grad_wsig, gr.d_grad_wout = _ptr(g_wh), _ptr(g_wsig), _ptr(g_wout)
             gr.d_grad_sky, gr.d_grad_sky_avg, gr.d_workspace = _ptr(g_sky), _ptr(g_sky_avg), _ptr(wsb)
-            _lib.check(L.sdb_render_rays_backward(ctypes.byref(prm), _ptr(ctx.record), ctypes.byref(gr), _stream(dev)),
-                       'sdb_render_rays_backward')
+            vg.w1ext_stride, vg.wh_stride, vg.wsig_stride = g_w1ext.stride(0), g_wh.stride(0), g_wsig.stride(0)
+            vg.wout_stride, vg.sky_avg_stride = g_wout.stride(0), g_sky_avg.stride(0)
+            _lib.check(L.sdb_render_rays_backward_views(ctypes.byref(prm), _ptr(ctx.record), ctypes.byref(vg), _stream(dev)),
+                       'sdb_render_rays_backward_views')
         # stream-ordered reuse: the next forward / backward run on the same stream after these kernels
         _give_scratch(wsb, 'bwd')
         _give_scratch(ctx.record, 'record')
         ctx.record = None
-        s_fcma, s_wsig, s_bsig, s_sky, s_skyavg, s_genc = ctx.shapes
+        s_fcma, s_wsig, s_bsig, s_sky, s_skyavg, s_genc, s_wh, s_bh = ctx.shapes
         n_lab = s_fcma[1]
         d_genc = torch.zeros(s_genc, dtype=torch.float32, device=dev)
         d_genc.view(-1)[:2] = g_genc
         return (None, g_table, d_genc,
-                g_w1ext[:, :128].contiguous(), g_w1ext[:, 143].contiguous(), g_w1ext[:, 128:128 + n_lab].contiguous(),
-                g_wh[:, :, :256].contiguous(), g_wh[:, :, 256].contiguous(),
-                g_wsig[0, :256].reshape(s_wsig), g_wsig[0, 256].reshape(s_bsig),
-                g_wout[:, :256].contiguous(), g_wout[:, 256].contiguous(),
+                _view_sum(g_w1ext[:, :, :128]).contiguous(), _view_sum(g_w1ext[:, :, 143]).contiguous(),
+                _view_sum(g_w1ext[:, :, 128:128 + n_lab]).contiguous(),
+                g_wh[:, :, :, :256].reshape(s_wh), g_wh[:, :, :, 256].reshape(s_bh),
+                _view_sum(g_wsig[:, 0, :256]).reshape(s_wsig), _view_sum(g_wsig[:, 0, 256]).reshape(s_bsig),
+                _view_sum(g_wout[:, :, :256]).contiguous(), _view_sum(g_wout[:, :, 256]).contiguous(),
                 g_sky.reshape(s_sky), g_sky_avg.reshape(s_skyavg))
 
 
 class _SkyTrainFn(torch.autograd.Function):
-    """sky [1,H,W,64] = SKYMLP(PE(raydirs)) on the wgmma engine, differentiable w.r.t. the weights.
-    b1 is the effective layer-0 bias fc1.bias + fc_z_a(z) (gancraft_base.py:159-160), formed by the caller in torch."""
+    """sky [N,H,W,64] = SKYMLP(PE(raydirs)) on the wgmma engine, differentiable w.r.t. the weights.
+    b1 [N,256] is each view's effective layer-0 bias fc1.bias + fc_z_a(z) (gancraft_base.py:159-160), formed by the caller in
+    torch; the other weights are shared by the views and get the sum of their gradients."""
 
     @staticmethod
     def forward(ctx, raydirs, w1, b1, wh, bh, wout, bout):
         L = _lib.lib()
         dev = raydirs.device
         N, H, W = raydirs.shape[:3]
-        if N != 1:
-            raise RuntimeError('fused sky training path renders one view per call')
+        if b1.numel() != N * 256:
+            raise RuntimeError('fused sky training path: b1 needs one [256] bias per view')
         f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()
-        w1_, b1_, wh_, bh_, wout_, bout_ = f32(w1), f32(b1).reshape(-1), f32(wh), f32(bh), f32(wout), f32(bout)
+        w1_, b1_, wh_, bh_, wout_, bout_ = f32(w1), f32(b1).reshape(N, 256), f32(wh), f32(bh), f32(wout), f32(bout)
         rd = raydirs.detach().contiguous()
         with torch.cuda.device(dev):
-            pack = torch.empty(int(L.sdb_sky_pack_bytes(PRECISION_FP16X3)), dtype=torch.uint8, device=dev)
-            _lib.check(L.sdb_pack_sky_mlp(_ptr(w1_), _ptr(b1_), _ptr(wh_), _ptr(bh_), _ptr(wout_), _ptr(bout_), PRECISION_FP16X3,
-                                          _ptr(pack), _stream(dev)), 'sdb_pack_sky_mlp')
+            pack = torch.empty(N, int(L.sdb_sky_pack_bytes(PRECISION_FP16X3)), dtype=torch.uint8, device=dev)      # one per view
+            for i in range(N):
+                _lib.check(L.sdb_pack_sky_mlp(_ptr(w1_), _ptr(b1_[i]), _ptr(wh_), _ptr(bh_), _ptr(wout_), _ptr(bout_),
+                                              PRECISION_FP16X3, _ptr(pack[i]), _stream(dev)), 'sdb_pack_sky_mlp')
             sky = torch.empty(N, H, W, 64, dtype=torch.float32, device=dev)
             avg = torch.empty(N, 64, dtype=torch.float32, device=dev)
             ws = torch.empty(int(L.sdb_sky_workspace_bytes(N, H, W)), dtype=torch.uint8, device=dev)
             record = _take_scratch(L.sdb_sky_train_record_bytes(N, H, W), dev, 'sky_record')
-            _lib.check(L.sdb_sky_train_forward(_ptr(rd), N, H, W, _ptr(pack), _ptr(sky), _ptr(avg), _ptr(ws), _ptr(record),
-                                               _stream(dev)), 'sdb_sky_train_forward')
+            _lib.check(L.sdb_sky_train_forward_views(_ptr(rd), N, H, W, _ptr(pack), int(pack.stride(0)), _ptr(sky), _ptr(avg),
+                                                     _ptr(ws), _ptr(record), _stream(dev)), 'sdb_sky_train_forward_views')
         ctx.dims, ctx.record, ctx.saved = (N, H, W), record, (wh_, wout_)
         ctx.shapes = (tuple(b1.shape),)
         return sky
@@ -596,23 +621,26 @@ class _SkyTrainFn(torch.autograd.Function):
         with torch.cuda.device(dev):
             bpack = torch.empty(int(L.sdb_sky_backward_pack_bytes()), dtype=torch.uint8, device=dev)
             _lib.check(L.sdb_pack_sky_mlp_backward(_ptr(wh_), _ptr(wout_), _ptr(bpack), _stream(dev)), 'sdb_pack_sky_mlp_backward')
-            g_w1ext = torch.empty(256, 48, dtype=torch.float32, device=dev)
-            g_wh = torch.empty(4, 256, 272, dtype=torch.float32, device=dev)
-            g_wout = torch.empty(64, 272, dtype=torch.float32, device=dev)
+            g_w1ext = torch.empty(N, 256, 48, dtype=torch.float32, device=dev)
+            g_wh = torch.empty(N, 4, 256, 272, dtype=torch.float32, device=dev)
+            g_wout = torch.empty(N, 64, 272, dtype=torch.float32, device=dev)
             wsb = _take_scratch(L.sdb_sky_backward_workspace_bytes(N, H, W), dev, 'sky_bwd')
-            _lib.check(L.sdb_sky_backward(N, H, W, _ptr(ctx.record), _ptr(g), _ptr(bpack), _ptr(g_w1ext), _ptr(g_wh), _ptr(g_wout),
-                                          _ptr(wsb), _stream(dev)), 'sdb_sky_backward')
+            vg = _SkyViewGrads(_ptr(g_w1ext), g_w1ext.stride(0), _ptr(g_wh), g_wh.stride(0), _ptr(g_wout), g_wout.stride(0))
+            _lib.check(L.sdb_sky_backward_views(N, H, W, _ptr(ctx.record), _ptr(g), _ptr(bpack), 0, ctypes.byref(vg), _ptr(wsb),
+                                                _stream(dev)), 'sdb_sky_backward_views')
         _give_scratch(wsb, 'sky_bwd')
         _give_scratch(ctx.record, 'sky_record')
         ctx.record = None
-        return (None, g_w1ext[:, :33].contiguous(), g_w1ext[:, 47].reshape(ctx.shapes[0]), g_wh[:, :, :256].contiguous(),
-                g_wh[:, :, 256].contiguous(), g_wout[:, :256].contiguous(), g_wout[:, 256].contiguous())
+        return (None, _view_sum(g_w1ext[:, :, :33]).contiguous(), g_w1ext[:, :, 47].reshape(ctx.shapes[0]),
+                _view_sum(g_wh[:, :, :, :256]).contiguous(), _view_sum(g_wh[:, :, :, 256]).contiguous(),
+                _view_sum(g_wout[:, :, :256]).contiguous(), _view_sum(g_wout[:, :, 256]).contiguous())
 
 
 def sky_features_train(P, raydirs, z, prefix='sky_net'):
-    """Differentiable a9 on the tensor-core engine: gradients reach P['sky_net.*'] and z [1,256]."""
+    """Differentiable a9 on the tensor-core engine for N views: gradients reach P['sky_net.*'] and z [N,256]."""
     p = prefix + '.'
-    b1 = P[p + 'fc1.bias'] + F.linear(z, P[p + 'fc_z_a.weight'])[0]                       # gancraft_base.py:159-160
+    # gancraft_base.py:159-160, [N,256]; view by view, so that a batch forms each bias exactly as a single-view call does
+    b1 = P[p + 'fc1.bias'] + torch.cat([F.linear(z[i:i + 1], P[p + 'fc_z_a.weight']) for i in range(z.shape[0])])
     wh = torch.stack([P[p + 'fc%d.weight' % k] for k in (2, 3, 4, 5)])
     bh = torch.stack([P[p + 'fc%d.bias' % k] for k in (2, 3, 4, 5)])
     return _SkyTrainFn.apply(raydirs, P[p + 'fc1.weight'], b1, wh, bh, P[p + 'fc_out_c.weight'], P[p + 'fc_out_c.bias'])
@@ -620,18 +648,28 @@ def sky_features_train(P, raydirs, z, prefix='sky_net'):
 
 def render_rays_train(P, voxel_id, depth2, raydirs, cam_ori, z, global_enc, voxel_dims, label_lut, per_level_scale,
                       num_samples=24, sample_depth=3.0, dists_scale=0.25, uniforms=None, base_res=16, log2_T=19, L=16,
-                      prefix='render_net', sky_prefix='sky_net', sky_impl='native'):
-    """Differentiable fused a2-a12 for ONE view: gradients reach P['hash_encoder.embeddings'], P['render_net.*'],
-    P['sky_net.*'], z [1,256] and global_enc [1,2] (everything Generator._forward_perpix differentiates under train.py).
+                      prefix='render_net', sky_prefix='sky_net', sky_impl='native', sky_avg=None):
+    """Differentiable fused a2-a12 for N views of ONE scene in one recorded pass (voxel_id [N,H,W,M,1], z [N,256],
+    global_enc [1,2] or N equal rows): gradients reach P['hash_encoder.embeddings'], P['render_net.*'], P['sky_net.*'], z
+    and global_enc (everything Generator._forward_perpix differentiates under train.py), summed over the views as autograd
+    sums them.  sky_avg: None = each view's own frame mean of its sky features (scenedreamer.py:395), else a caller-supplied
+    mean [N or 1, 64] used as every view's (scenedreamer.py:391-392; differentiable when it requires grad).
     sky_impl: 'native' = the sky branch on the tensor-core engine too (sky_features_train), 'torch' = torch autograd /
     cuBLAS fp32 on top of the PE kernel (independent cross-check)."""
     p = prefix + '.'
-    wh, bh = modulated_weights(P, z[0], prefix)                            # differentiable w.r.t. P and z
+    N = voxel_id.shape[0]
+    if z.shape[0] != N:
+        raise ValueError('render_rays_train: z needs one style code per view (%d), got %d' % (N, z.shape[0]))
+    mods = [modulated_weights(P, z[i], prefix) for i in range(N)]          # differentiable w.r.t. P and z
+    wh, bh = torch.stack([m[0] for m in mods]), torch.stack([m[1] for m in mods])
     if sky_impl == 'native':
-        sky = sky_features_train(P, raydirs, z, prefix=sky_prefix)         # [1,H,W,64]
+        sky = sky_features_train(P, raydirs, z, prefix=sky_prefix)         # [N,H,W,64]
     else:
         sky = sky_features(P, raydirs, z, prefix=sky_prefix)
-    sky_avg = sky.mean(dim=(1, 2))                                         # scenedreamer.py:395
+    if sky_avg is None:                                                    # scenedreamer.py:395, view by view: the same reduction
+        sky_avg = torch.cat([sky[i:i + 1].mean(dim=(1, 2)) for i in range(N)]) if N > 1 else sky.mean(dim=(1, 2))  # as one view
+    else:
+        sky_avg = sky_avg.reshape(-1, 64).expand(N, 64)
     cfg = dict(voxel_id=voxel_id, depth2=depth2, raydirs=raydirs, cam_ori=cam_ori, lut=label_lut, voxel_dims=voxel_dims,
                num_samples=num_samples, sample_depth=sample_depth, dists_scale=dists_scale, uniforms=uniforms,
                per_level_scale=per_level_scale, base_res=base_res, log2_T=log2_T, L=L)
