@@ -226,6 +226,8 @@ def _cumsum_seq(x, dim):
         xi = x.select(dim, i)
         acc = xi.clone() if acc is None else acc + xi
         outs.append(acc)
+    if not outs:                      # an empty scan (one voxel hit per ray: no gaps between hits) is empty, like torch.cumsum
+        return x.clone()
     return torch.stack(outs, dim=dim)
 
 

@@ -62,8 +62,12 @@ __device__ __forceinline__ Sample sample_at(const Params &p, const float *st, in
         r0 = __fmul_rn(frac[k], total);
         r1 = __fmul_rn(frac[k + 1], total);
     } else {                              // stratified: (u / nsamples + k / nsamples) * total (:122-126)
+        // a ray without intervals samples at 0 whatever u is; rows of a tile outside the image are such rays, and their `ray`
+        // lies past the image (past the end of the uniforms for the last one), so their u is not read
         const float ns = (float)(p.S + 1);
-        const float u0 = __ldg(p.uniforms + ray * (p.S + 1) + k), u1 = __ldg(p.uniforms + ray * (p.S + 1) + k + 1);
+        const bool any = total > 0.0f;
+        const float u0 = any ? __ldg(p.uniforms + ray * (p.S + 1) + k) : 0.0f;
+        const float u1 = any ? __ldg(p.uniforms + ray * (p.S + 1) + k + 1) : 0.0f;
         r0 = __fmul_rn(__fadd_rn(__fdiv_rn(u0, ns), frac[k]), total);
         r1 = __fmul_rn(__fadd_rn(__fdiv_rn(u1, ns), frac[k + 1]), total);
     }

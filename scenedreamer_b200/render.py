@@ -548,7 +548,7 @@ class _FusedRenderTrainFn(torch.autograd.Function):
             g_wh = torch.empty(N, 5, 256, 272, dtype=torch.float32, device=dev)
             g_wsig = torch.empty(N, 8, 272, dtype=torch.float32, device=dev)
             g_wout = torch.empty(N, 64, 272, dtype=torch.float32, device=dev)
-            g_sky = torch.zeros(N, H, W, 64, dtype=torch.float32, device=dev)
+            g_sky = torch.empty(N, H, W, 64, dtype=torch.float32, device=dev)      # every ray's is written (sdb200.h)
             g_sky_avg = torch.empty(N, 64, dtype=torch.float32, device=dev)
             wsb = _take_scratch(L.sdb_render_backward_workspace_bytes(N, H, W, S, int(cfg['L']), int(cfg['log2_T'])), dev, 'bwd')
             vg = _RenderViewGrads()

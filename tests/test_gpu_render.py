@@ -29,13 +29,18 @@ def lut(golden_ops):
     return render.reduced_label_lut(golden_ops['mc2reduced_lut'], 0, 3)
 
 
-@pytest.fixture(scope='module')
-def scene():
+def make_scene(M=6):
+    """The test frame with up to M voxel hits per ray (the kernels take 1 <= M <= 8)."""
     world = synth.SyntheticVoxelWorld(size=128, seed=7)
     pose = synth.eval_camera_poses(world, maxstep=8, pattern=0)[1]
     o, d, u, f, c, res = synth.frame_camera(world, pose, resolution_hw=(44, 60), pad=4)
-    vid, dep, rd = ops.ray_voxel_intersection_perspective(world.voxel_t.to(DEV), o, d, u, f, c, res, 6)
+    vid, dep, rd = ops.ray_voxel_intersection_perspective(world.voxel_t.to(DEV), o, d, u, f, c, res, M)
     return dict(world=world, o=o, vid=vid.unsqueeze(0), dep=dep.unsqueeze(0), rd=rd.unsqueeze(0))
+
+
+@pytest.fixture(scope='module')
+def scene():
+    return make_scene()
 
 
 def run_oracle(P, sc, z, genc, lut_raw, S=24, uniforms=None):
@@ -123,12 +128,16 @@ def test_fused_stratified_sampling_and_small_S(scene, lut, golden_ops):
     z = oracle.style_mlp(torch.randn(1, 128, generator=g), P)
     genc = torch.tanh(torch.randn(1, 2, generator=g))
     N, H, W = scene['vid'].shape[:3]
-    for S in (24, 4):
+    scenes = {6: scene, 1: make_scene(1), 8: make_scene(8)}
+    # bf16x3 (2^-16 per product) at S = 24 and 4; the other inputs at the fp16x3 default: at S = 1 one sample carries the
+    # whole output and nothing averages its error, which in bf16x3 reaches the bar (1.02e-3 measured, 6.8e-5 in fp16x3)
+    bf, fp = render.PRECISION_BF16X3, render.PRECISION_FP16X3
+    for S, M, prec in ((24, 6, bf), (4, 6, bf), (1, 6, fp), (33, 6, fp), (64, 6, fp), (24, 1, fp), (33, 8, fp)):
         u = torch.rand(N, H, W, S + 1, 1, generator=g)
-        ref = run_oracle(P, scene, z, genc, torch.from_numpy(golden_ops['mc2reduced_lut']), S=S, uniforms=u)
-        out = run_fused(P, scene, z, genc, lut, render.PRECISION_BF16X3, False, S=S, uniforms=u)
+        ref = run_oracle(P, scenes[M], z, genc, torch.from_numpy(golden_ops['mc2reduced_lut']), S=S, uniforms=u)
+        out = run_fused(P, scenes[M], z, genc, lut, prec, False, S=S, uniforms=u)
         err = (out['net_out'].cpu() - ref['net_out']).abs()
-        print('stratified S=%d: net_out max err %.3e' % (S, float(err.max())))
+        print('stratified S=%d M=%d precision %d: net_out max err %.3e' % (S, M, prec, float(err.max())))
         assert float(err.max()) <= TOL
 
 
@@ -235,7 +244,8 @@ def test_early_termination_error_bound_and_savings(scene, lut, golden_ops):
 def test_ray_slots_equal_the_tile_kernel(scene, lut, golden_ops, monkeypatch):
     """The ray-slot kernel (every MMA row a ray with its own cursor, the inference default) against the tile kernel
     (SDB_RAY_SLOTS=0): bit-identical with early termination off -- every ray's arithmetic is the same, only its row and
-    its companions differ -- and within the termination threshold otherwise."""
+    its companions differ -- and within the termination threshold otherwise.  Bit-identity also at S = 64 and with M = 1
+    and 8 voxel hits per ray."""
     P = oracle.make_params(seed=21, stress=True)
     P['render_net.fc_sigma.bias'] = torch.full((1,), 60.0)
     g = torch.Generator().manual_seed(8888)
@@ -257,6 +267,18 @@ def test_ray_slots_equal_the_tile_kernel(scene, lut, golden_ops, monkeypatch):
             res[(T, variant)] = ({k: o[k].clone() for k in keys}, int(ws[1]))
     for k in keys:
         assert torch.equal(res[(0.0, '1')][0][k], res[(0.0, '0')][0][k]), k
+    r.early_stop = 0.0
+    for S, M in ((64, 6), (24, 1), (33, 8), (1, 8)):
+        sc = scene if M == 6 else make_scene(M)
+        same = {}
+        for variant in ('1', '0'):
+            monkeypatch.setenv('SDB_RAY_SLOTS', variant)
+            o = r.forward(sc['vid'], sc['dep'], sc['rd'], sc['o'].unsqueeze(0), z.to(DEV), genc.to(DEV), num_samples=S,
+                          want_samples=True)
+            torch.cuda.synchronize()
+            same[variant] = {k: o[k].clone() for k in keys}
+        for k in keys:
+            assert torch.equal(same['1'][k], same['0'][k]), (S, M, k)
     a, b = res[(None, '1')][0], res[(None, '0')][0]
     assert float((a['net_out'] - b['net_out']).abs().max()) <= 5 * render.EARLY_STOP_T
     assert torch.equal(a['rand_depth'], b['rand_depth'])

@@ -31,13 +31,17 @@ def device_level_scales(L, pls, base):
     return (torch.exp2(lv * S) * float(base) - 1.0).cpu()
 
 
-@pytest.fixture(scope='module')
-def scene():
+def make_scene(M=6):
     world = synth.SyntheticVoxelWorld(size=128, seed=7)
     pose = synth.eval_camera_poses(world, maxstep=8, pattern=0)[1]
     o, d, u, f, c, res = synth.frame_camera(world, pose, resolution_hw=(36, 52), pad=4)
-    vid, dep, rd = ops.ray_voxel_intersection_perspective(world.voxel_t.to(DEV), o, d, u, f, c, res, 6)
+    vid, dep, rd = ops.ray_voxel_intersection_perspective(world.voxel_t.to(DEV), o, d, u, f, c, res, M)
     return dict(world=world, o=o, vid=vid.unsqueeze(0), dep=dep.unsqueeze(0), rd=rd.unsqueeze(0))
+
+
+@pytest.fixture(scope='module')
+def scene():
+    return make_scene()
 
 
 def _leaf(P, dev):
@@ -52,9 +56,9 @@ GRAD_KEYS = ['hash_encoder.embeddings', 'render_net.fc_1.weight', 'render_net.fc
                                                                                 'weight_beta', 'bias_beta')]
 
 
-@pytest.mark.parametrize('stress,S,stratified', [(True, 24, True), (False, 12, False)])
-def test_fused_backward_vs_oracle_autograd(scene, golden_ops, stress, S, stratified):
-    sc = scene
+@pytest.mark.parametrize('stress,S,stratified,M', [(True, 24, True, 6), (False, 12, False, 6), (True, 64, True, 8)])
+def test_fused_backward_vs_oracle_autograd(scene, golden_ops, stress, S, stratified, M):
+    sc = scene if M == 6 else make_scene(M)
     P0 = oracle.make_params(seed=21, stress=stress)
     g = torch.Generator().manual_seed(8888)
     z0 = oracle.style_mlp(torch.randn(1, 128, generator=g), P0)
