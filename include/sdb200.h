@@ -263,10 +263,14 @@ int sdb_sky_forward(const float *d_raydirs, int32_t n_img, int32_t H, int32_t W,
 
 /* --------------------------------------------------------------------------------------------
  * a7 + backward of a8/a10/a11: training.  sdb_render_rays_train_forward is sdb_render_rays_forward
- * (fp16x3, pre-blended table: p->d_table3, p->precision == 2) that additionally writes a RECORD of
- * the pass into caller-owned device memory: per-sample hash-grid coordinates and features, the six
- * hidden activations (bf16) with their LeakyReLU sign words, sigma, interval length and the colour
- * head output.  sdb_render_rays_backward turns dL/d net_out into every parameter gradient of the
+ * (pre-blended table: p->d_table3, no early termination) that additionally writes a RECORD of the
+ * pass into caller-owned device memory.  Accepted precisions (the pack must have been made with the
+ * same): 2 = fp16 x3, fp32-grade, the default; 0 = one fp16 pass with fp32 accumulation, the class of
+ * torch.autocast's fp16 matmuls (mixed-precision training); 1 returns SDB_EUNSUPPORTED.  Both modes
+ * write the same record from the fp32 values their pass computed, and the backward (bf16 x3) is the
+ * same for both: it takes the forward's params whatever their precision.  The record holds per-sample
+ * hash-grid coordinates and features, the six hidden activations (bf16) with their LeakyReLU sign
+ * words, sigma, interval length and the colour head output.  sdb_render_rays_backward turns dL/d net_out into every parameter gradient of the
  * per-pixel path -- what torch.autograd produces for Generator._forward_perpix in the reference
  * (imaginaire/generators/scenedreamer.py:313-428 under train.py; kernel_grid_backward /
  * kernel_input_backward gridencoder.cu:227-343 for the table and the scene code):
@@ -312,7 +316,7 @@ int64_t sdb_render_backward_workspace_bytes(int32_t n_img, int32_t H, int32_t W,
 int sdb_render_rays_backward(const sdb_render_params *p, const void *d_record, const sdb_render_grads *g, void *stream);
 
 /* A batch of views of ONE scene in one recorded pass.  sdb_render_rays_train_forward takes n_img >= 1 views: one pack per
- * view through mlp_pack_stride (0 = shared; else >= sdb_mlp_pack_bytes(2)), d_sky_avg [n_img, 64], and d_table3 of the one
+ * view through mlp_pack_stride (0 = shared; else >= sdb_mlp_pack_bytes(precision)), d_sky_avg [n_img, 64], and d_table3 of the one
  * scene code all views share (the caller checks that their global_enc are equal).  Its record
  * (sdb_render_train_record_bytes(n_img, ...)) lists the live tiles grouped by image and keeps per image {first list
  * position, live tiles} in its header, on the device; with n_img == 1 its layout is the single-view one.

@@ -1426,7 +1426,9 @@ int launch_mlp(const Params &p_in, int grid, cudaStream_t st) {
     return SDB_OK;
 }
 
-int launch_train_forward(const Params &p, int grid, cudaStream_t st) { return launch_mlp<2, false, kRender, true>(p, grid, st); }
+int launch_train_forward(const Params &p, int precision, int grid, cudaStream_t st) {
+    return precision == 0 ? launch_mlp<0, false, kRender, true>(p, grid, st) : launch_mlp<2, false, kRender, true>(p, grid, st);
+}
 int launch_bwd_chain(const Params &p, int grid, cudaStream_t st) { return launch_mlp<1, false, kBwd>(p, grid, st); }
 int launch_sky_train_forward(const Params &p, int grid, cudaStream_t st) { return launch_mlp<2, false, kSky, true>(p, grid, st); }
 int launch_sky_bwd_chain(const Params &p, int grid, cudaStream_t st) { return launch_mlp<1, false, kSkyBwd>(p, grid, st); }

@@ -400,8 +400,10 @@ extern "C" int sdb_render_rays_train_forward(const sdb_render_params *sp, void *
         const int rc = params_from_abi(sp, p);
         if (rc != SDB_OK) return rc;
     }
-    if (p.raw5d || sp->precision != 2) return SDB_EUNSUPPORTED;      // record + backward are built on the pre-blended table, fp16x3
-    if (p.n_img > 1 && (p.pack_stride < 0 || (p.pack_stride > 0 && p.pack_stride < packBytes<kRender>(2)))) return SDB_EINVAL;
+    // record + backward are built on the pre-blended table; the forward runs fp16 x3 or, for mixed precision, one fp16 pass
+    if (p.raw5d || sp->precision == 1) return SDB_EUNSUPPORTED;
+    const int parts = sp->precision == 0 ? 1 : 2;
+    if (p.n_img > 1 && (p.pack_stride < 0 || (p.pack_stride > 0 && p.pack_stride < packBytes<kRender>(parts)))) return SDB_EINVAL;
     uint8_t *rec = (uint8_t *)d_record;
     const RecordLayout rl = record_layout(p.n_img, p.n_tiles, p.S);
     bind_record(p, rec, rl);
@@ -410,7 +412,7 @@ extern "C" int sdb_render_rays_train_forward(const sdb_render_params *sp, void *
         if (rc != SDB_OK) return rc;
     }
     const int grid = p.n_tiles < sdb_num_sms() ? p.n_tiles : sdb_num_sms();
-    return launch_train_forward(p, grid, st);
+    return launch_train_forward(p, sp->precision, grid, st);
 }
 
 // gradient strides between images, in floats: w1ext, wh, wsig, wout, sky_avg (one image's size each when n_img == 1)

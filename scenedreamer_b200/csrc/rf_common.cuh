@@ -326,7 +326,7 @@ static inline SkyBwdLayout sky_bwd_layout(long long n_tiles) {
 }
 
 // launchers implemented in render_fused.cu, used by render_train.cu
-int launch_train_forward(const Params &p, int grid, cudaStream_t st);     // mlp_kernel<fp16x3, table3, kRender, TRAIN>
+int launch_train_forward(const Params &p, int precision, int grid, cudaStream_t st);     // mlp_kernel<fp16 x1 | x3, table3, kRender, TRAIN>
 int launch_bwd_chain(const Params &p, int grid, cudaStream_t st);         // mlp_kernel<bf16x3, -, kBwd>
 int launch_sky_train_forward(const Params &p, int grid, cudaStream_t st); // mlp_kernel<fp16x3, -, kSky, TRAIN>
 int launch_sky_bwd_chain(const Params &p, int grid, cudaStream_t st);     // mlp_kernel<bf16x3, -, kSkyBwd>

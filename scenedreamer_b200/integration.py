@@ -121,9 +121,11 @@ class _FusedState:
         return self.cnn
 
     def get_renderer(self, gen):
+        precision = precision_for(self)
         # inside an epoch (one public call of the generator) the weights cannot change behind torch's back: the state-dict scan
         # below is done once per epoch, not once per tile of the reference's tile loop (40 scans x ~0.3 ms per frame)
-        if self.renderer is not None and self.renderer_epoch == self.epoch and not torch.is_grad_enabled():
+        if self.renderer is not None and self.renderer_epoch == self.epoch and not torch.is_grad_enabled() and \
+                self.renderer.precision == precision:
             return self.renderer
         self.renderer_epoch = self.epoch
         mods = (('render_net', gen.render_net), ('sky_net', gen.sky_net), ('hash_encoder', gen.hash_encoder))
@@ -133,11 +135,11 @@ class _FusedState:
                 P[prefix + '.' + k] = v
         dims = tuple(gen.voxel.voxel_t.shape)
         # state_dict() hands out detached aliases: identity is the storage, _version is shared with the Parameter
-        key = (self.epoch, dims, tuple((k, v.data_ptr(), v._version) for k, v in P.items()))
+        key = (self.epoch, precision, dims, tuple((k, v.data_ptr(), v._version) for k, v in P.items()))
         if self.renderer_key != key:
             he = gen.hash_encoder
             self.renderer = render.FusedPerPixelRenderer(
-                P, dims, self.lut, he.per_level_scale, precision=self.precision, preblend=True,
+                P, dims, self.lut, he.per_level_scale, precision=precision, preblend=True,
                 base_res=he.base_resolution, log2_T=he.log2_hashmap_size, L=he.num_levels)
             self.renderer_key = key
         return self.renderer
@@ -171,11 +173,10 @@ def _live_params(gen):
 # ------------------------------------------------------------------------------------------------
 def supported(gen, voxel_id, z, global_enc):
     """The fused path covers what both SceneDreamer configs use (configs/scenedreamer_{train,inference}.yaml):
-    no view-direction input to the MLP, segmentation labels on, clipped feature blending, global sky average, AMP off (under
-    autocast the reference composition runs instead, over the drop-in ops -- the grid encoder then takes its float16 table path)."""
+    no view-direction input to the MLP, segmentation labels on, clipped feature blending, global sky average; with AMP on or
+    off (precision_for)."""
     rn = gen.render_net
     return bool(
-        not torch.is_autocast_enabled() and
         z is not None and global_enc is not None and voxel_id.is_cuda and
         gen.clip_feat_map is True and gen.keep_sky_out and gen.keep_sky_out_avgpool and gen.sky_global_avgpool and
         not gen.sample_use_box_boundaries and gen.raw_noise_std == 0 and
@@ -185,6 +186,14 @@ def supported(gen, voxel_id, z, global_enc):
         getattr(gen.hash_encoder, 'input_dim', 5) == 5 and getattr(gen.hash_encoder, 'level_dim', 8) == 8 and
         getattr(gen.hash_encoder, 'gridtype', 'hash') == 'hash' and not getattr(gen.hash_encoder, 'align_corners', False) and
         global_enc.shape[-1] == 2)
+
+
+def precision_for(st):
+    """MLP precision of a fused per-pixel call.  Under autocast (fp16 or bf16: fp16 operands are the finer of the two, and
+    the default mode already assumes fp16's range) one fp16 tensor-core pass with fp32 accumulation -- the class of autocast's
+    own fp16 matmuls; otherwise the generator's precision (fp16 x3 by default).  The sky branch and the backward stay
+    fp32-grade in both (DESIGN.md section 3.5)."""
+    return render.PRECISION_FP16 if torch.is_autocast_enabled() else st.precision
 
 
 def _needs_grad(gen, z, global_enc):
@@ -261,6 +270,7 @@ def fused_forward_perpix(self, blk_feats, voxel_id, depth2, raydirs, cam_ori_t, 
         st.stats['reference_calls'] += 1
         return reference(self, blk_feats, voxel_id, depth2, raydirs, cam_ori_t, z, global_enc)
     needs_grad = _needs_grad(self, z, global_enc)
+    prec = precision_for(st)
     N, H, W = voxel_id.shape[:3]
     train_views = train_views_enabled()
     if needs_grad:
@@ -286,7 +296,7 @@ def fused_forward_perpix(self, blk_feats, voxel_id, depth2, raydirs, cam_ori_t, 
         sky_attr = getattr(self, 'sky_avg', None)
         sky_avg = None if sky_attr is None else sky_attr.reshape(-1, 64).expand(N, 64)
         args = ([float(v) for v in self.voxel.voxel_t.shape], st.lut, he.per_level_scale)
-        kw.update(base_res=he.base_resolution, log2_T=he.log2_hashmap_size, L=he.num_levels)
+        kw.update(base_res=he.base_resolution, log2_T=he.log2_hashmap_size, L=he.num_levels, precision=prec)
         if train_views:
             out = render.render_rays_train(P, voxel_id.contiguous(), depth2.contiguous(), raydirs.contiguous(), cam_ori_t, z,
                                            global_enc[:1], *args, uniforms=uniforms, sky_avg=sky_avg, **kw)
@@ -300,24 +310,30 @@ def fused_forward_perpix(self, blk_feats, voxel_id, depth2, raydirs, cam_ori_t, 
     st.stats['fused_calls'] += 1
     r = st.get_renderer(self)
     sky_attr = getattr(self, 'sky_avg', None)                  # set once per frame by inference_givenstyle (scenedreamer.py:592-598)
-    sky_avg = sky_attr.reshape(-1, 64) if sky_attr is not None else None
+    sky_avg = sky_attr.reshape(-1, 64).float() if sky_attr is not None else None
+    # under autocast z, global_enc and a preset sky_avg arrive in fp16: the packers and kernels take them in fp32, and the torch
+    # glue of the renderer (style fold, sky mean) runs in fp32 too
+    zf, gencf = z.float(), global_enc.float()
+    no_autocast = torch.autocast('cuda', enabled=False)
     win = _frame_window(voxel_id, depth2, raydirs) if (N == 1 and uniforms is None) else None
     if win is not None:
         bases, h0, w0, h, w = win
         # keyed on the tensor OBJECTS the tile loop hands over unchanged from tile to tile (a reshape would be a new object)
         keyt = list(bases) + [z, global_enc] + ([sky_attr] if sky_attr is not None else [])
-        full, key = st.frame.lookup(keyt, st.epoch, (self.num_samples, float(self.sample_depth), float(self.dists_scale)))
+        full, key = st.frame.lookup(keyt, st.epoch, (self.num_samples, float(self.sample_depth), float(self.dists_scale), prec))
         if full is None:
             st.stats['frame_launches'] += 1
-            full = r.forward(bases[0].unsqueeze(0), bases[1].unsqueeze(0), bases[2].unsqueeze(0), cam_ori_t, z, global_enc,
-                             sky_avg=sky_avg, want_samples=True, **kw)
+            with no_autocast:
+                full = r.forward(bases[0].unsqueeze(0), bases[1].unsqueeze(0), bases[2].unsqueeze(0), cam_ori_t, zf, gencf,
+                                 sky_avg=sky_avg, want_samples=True, **kw)
             st.frame.store(key, keyt, full)
         else:
             st.stats['tile_hits'] += 1
         out = {k: full[k][:, h0:h0 + h, w0:w0 + w] for k in ('net_out', 'total_weight', 'weights', 'rand_depth', 'sky')}
         return _tuple12(out, sky_mask, sky_only_mask)
-    out = r.forward(voxel_id.contiguous(), depth2.contiguous(), raydirs.contiguous(), cam_ori_t, z, global_enc,
-                    uniforms=uniforms, sky_avg=sky_avg, want_samples=True, **kw)
+    with no_autocast:
+        out = r.forward(voxel_id.contiguous(), depth2.contiguous(), raydirs.contiguous(), cam_ori_t, zf, gencf,
+                        uniforms=uniforms, sky_avg=sky_avg, want_samples=True, **kw)
     return _tuple12(out, sky_mask, sky_only_mask)
 
 

@@ -50,6 +50,13 @@ def _eligible(opt, group, p):
 def _step_pre_hook(opt, args, kwargs):
     if type(opt) is not torch.optim.Adam:
         return None
+    # Under torch.amp.GradScaler a plain Adam is stepped only when every gradient is finite, and after unscale_: the hook then
+    # sees the true gradients and is not called on a skipped step.  A fused Adam (`_step_supports_amp_scaling`) is stepped
+    # with its gradients still scaled, also on a step to be skipped: GradScaler hands it the scale and the inf flag as the
+    # optimizer attributes `grad_scale` / `found_inf` for the length of the call, and the fused kernel unscales and skips by
+    # itself.  Leave the table to it then.
+    if getattr(opt, 'grad_scale', None) is not None or getattr(opt, 'found_inf', None) is not None:
+        return None
     for group in opt.param_groups:
         for p in group['params']:
             if not _eligible(opt, group, p):

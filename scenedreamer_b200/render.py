@@ -494,7 +494,7 @@ class _FusedRenderTrainFn(torch.autograd.Function):
         sky_, sky_avg_ = f32(sky).reshape(N, H, W, 64), f32(sky_avg).reshape(N, 64)
         cam_ori = cfg['cam_ori'].to(dev, torch.float32).reshape(N, 3).contiguous()
         lut = cfg['lut'].to(dev, torch.int32).contiguous()
-        prec = PRECISION_FP16X3
+        prec = int(cfg['precision'])
         with torch.cuda.device(dev):
             pack = torch.empty(N, int(L.sdb_mlp_pack_bytes(prec)), dtype=torch.uint8, device=dev)      # one pack per view
             for i in range(N):
@@ -648,14 +648,26 @@ def sky_features_train(P, raydirs, z, prefix='sky_net'):
 
 def render_rays_train(P, voxel_id, depth2, raydirs, cam_ori, z, global_enc, voxel_dims, label_lut, per_level_scale,
                       num_samples=24, sample_depth=3.0, dists_scale=0.25, uniforms=None, base_res=16, log2_T=19, L=16,
-                      prefix='render_net', sky_prefix='sky_net', sky_impl='native', sky_avg=None):
+                      prefix='render_net', sky_prefix='sky_net', sky_impl='native', sky_avg=None, precision=PRECISION_FP16X3):
     """Differentiable fused a2-a12 for N views of ONE scene in one recorded pass (voxel_id [N,H,W,M,1], z [N,256],
     global_enc [1,2] or N equal rows): gradients reach P['hash_encoder.embeddings'], P['render_net.*'], P['sky_net.*'], z
     and global_enc (everything Generator._forward_perpix differentiates under train.py), summed over the views as autograd
     sums them.  sky_avg: None = each view's own frame mean of its sky features (scenedreamer.py:395), else a caller-supplied
     mean [N or 1, 64] used as every view's (scenedreamer.py:391-392; differentiable when it requires grad).
     sky_impl: 'native' = the sky branch on the tensor-core engine too (sky_features_train), 'torch' = torch autograd /
-    cuBLAS fp32 on top of the PE kernel (independent cross-check)."""
+    cuBLAS fp32 on top of the PE kernel (independent cross-check).
+    precision: of the recording forward's MLP, PRECISION_FP16X3 (fp32-grade) or PRECISION_FP16 (one fp16 pass, for
+    mixed-precision training); the sky branch and the backward are fp32-grade either way.  The torch glue runs in fp32 with
+    autocast off, whatever the caller's autocast state and the dtypes of z / global_enc / sky_avg; autograd hands their
+    gradients back in their own dtypes."""
+    with torch.autocast('cuda', enabled=False):
+        return _render_rays_train(P, voxel_id, depth2, raydirs, cam_ori, z.float(), global_enc.float(), voxel_dims, label_lut,
+                                  per_level_scale, num_samples, sample_depth, dists_scale, uniforms, base_res, log2_T, L, prefix,
+                                  sky_prefix, sky_impl, None if sky_avg is None else sky_avg.float(), precision)
+
+
+def _render_rays_train(P, voxel_id, depth2, raydirs, cam_ori, z, global_enc, voxel_dims, label_lut, per_level_scale, num_samples,
+                       sample_depth, dists_scale, uniforms, base_res, log2_T, L, prefix, sky_prefix, sky_impl, sky_avg, precision):
     p = prefix + '.'
     N = voxel_id.shape[0]
     if z.shape[0] != N:
@@ -672,7 +684,7 @@ def render_rays_train(P, voxel_id, depth2, raydirs, cam_ori, z, global_enc, voxe
         sky_avg = sky_avg.reshape(-1, 64).expand(N, 64)
     cfg = dict(voxel_id=voxel_id, depth2=depth2, raydirs=raydirs, cam_ori=cam_ori, lut=label_lut, voxel_dims=voxel_dims,
                num_samples=num_samples, sample_depth=sample_depth, dists_scale=dists_scale, uniforms=uniforms,
-               per_level_scale=per_level_scale, base_res=base_res, log2_T=log2_T, L=L)
+               per_level_scale=per_level_scale, base_res=base_res, log2_T=log2_T, L=L, precision=precision)
     net_out, depth, tw, wts, rdp = _FusedRenderTrainFn.apply(
         cfg, P['hash_encoder.embeddings'], global_enc, P[p + 'fc_1.weight'], P[p + 'fc_1.bias'], P[p + 'fc_m_a.weight'],
         wh, bh, P[p + 'fc_sigma.weight'], P[p + 'fc_sigma.bias'], P[p + 'fc_out_c.weight'], P[p + 'fc_out_c.bias'], sky,
