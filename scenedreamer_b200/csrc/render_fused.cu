@@ -25,10 +25,11 @@
 //     per-CTA buffer pair in global memory (L2-resident, ping-pong by layer parity) and the epilogue reads
 //     its rows from there; MMA and epilogue hand a layer over per 64-row block, so the epilogue of one row block
 //     runs while the MMAs of the other do;
-//   * bias, style beta and the label embedding ride in the GEMM: the operand has 16 extra K columns
+//   * fc_1's bias and the label embedding ride in layer 0's GEMM: its operand has 16 extra K columns
 //     (one-hot label + constant 1), the weight image carries bias / embedding rows there -- exactly
-//     the reference's fc_m_a(onehot) product -- so the epilogue is LeakyReLU + 16-bit split only;
-//   * the 16-bit activations stay on chip: ONE in-place 128x272 operand buffer in shared memory; the
+//     the reference's fc_m_a(onehot) product; the biases of the later layers (style beta included) are
+//     fp32 adds where the MMA warpgroup writes a block out, so the epilogue is LeakyReLU + 16-bit split only;
+//   * the 16-bit activations stay on chip: ONE in-place 128x256 operand buffer in shared memory; the
 //     per-sample L2 traffic is the table gather plus the accumulator round trip above;
 //   * precision: 0 = one fp16 pass; 1 / 2 = bf16 / fp16 "x3" split (x_hi*W_hi + x_lo*W_hi + x_hi*W_lo:
 //     ~2^-16 resp. ~2^-21 relative, i.e. fp32-grade for the 1e-3 parity bar); accumulation is fp32;
@@ -352,11 +353,14 @@ mlp_kernel(const Params p)
     constexpr Smem SM = smem_map(X3);
     constexpr int PARTS = X3 ? 2 : 1;
     constexpr int NH = Net<MODE>::NH, NL = Net<MODE>::NL;
+    static_assert(SM.total <= 232448, "shared memory map exceeds the 227 KB a CTA can have");
+    static_assert(Net<MODE>::NBIAS <= Net<kRender>::NBIAS, "bias table slot");
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t *sHhi = smem + SM.h_hi;
     uint8_t *sHlo = smem + SM.h_lo;
     uint8_t *sRing = smem + SM.ring;
     float *sF = reinterpret_cast<float *>(smem + SM.fsec);
+    float *sBias = reinterpret_cast<float *>(smem + SM.bias);
     float *sScale = reinterpret_cast<float *>(smem + SM.scales);
     float *sFrac = reinterpret_cast<float *>(smem + SM.frac);
     float *sSig = reinterpret_cast<float *>(smem + SM.sig);
@@ -439,14 +443,6 @@ mlp_kernel(const Params p)
         for (int i = tid; i < kLevels; i += kThreads) sScale[i] = exp2f(i * p.level_S) * p.base_res - 1.0f;   // gridencoder.cu:126
         for (int i = tid; i <= p.S; i += kThreads) sFrac[i] = p.fractions[i];
     }
-    // constant K-extension columns of the hidden operand: column 256 = 1.0 (bias), 257..271 = 0
-    for (int i = tid; i < 2 * kRows; i += kThreads) {
-        const int r = i & (kRows - 1), kc = kHidden / 8 + (i >> 7);
-        const uint4 one = make_uint4((i >> 7) == 0 ? one16<PREC>() : 0u, 0u, 0u, 0u);
-        *reinterpret_cast<uint4 *>(sHhi + tc05::chunk_off(kRows, r, kc)) = one;
-        if constexpr (X3) *reinterpret_cast<uint4 *>(sHlo + tc05::chunk_off(kRows, r, kc)) = make_uint4(0, 0, 0, 0);
-    }
-    tc05::fence_proxy_async_smem();
     __syncthreads();
     const uint32_t mask = SKY ? 0u : ((1u << p.log2_T) - 1u);
 
@@ -796,15 +792,28 @@ mlp_kernel(const Params p)
       // Numerics: every stage starts a fresh tensor-core sum that is added to the block's running sum in fp32 with round-to-
       // nearest, in stage order: the tensor core's own accumulation does not round to nearest, and over a whole x3 layer (up to
       // 51 chained MMAs) that moved the full-frame depth outside its parity bound.  Two accumulator sets alternate, so that the
-      // add and the ring-slot release of one stage overlap the MMAs of the next.
+      // add and the ring-slot release of one stage overlap the MMAs of the next.  Layers 1 .. NL-1 of the forward networks
+      // then add their fp32 bias (the pack's table: hi + lo of the 16-bit parts, what a bias K slab would have summed on the
+      // tensor core, exactly) with one more round-to-nearest add, so a hidden 32-column block is exactly two full stages.
       const int t = tid - kMmaWarp0 * 32;
       constexpr uint32_t kSlot = 16384, kSlabB = 1024 * PARTS;       // ring slot; one k16 slab of a 32-column block
+      constexpr bool BIAS = Net<MODE>::NBIAS > 0;
       uint32_t n = 0, q = 0, qr = 0;                                 // ring stages issued to the tensor cores / retired
+      int loaded_img = -1;
       for (int it = 0;; it++) {
           const int work = fetch_work(it);
           if (work < 0) break;
           const int tile = RAYQ ? 0 : (ONE_STEP ? work : p.tile_list[rec_work(work) / wmult]);
-          const uint8_t *pack = p.pack + (long long)tile_coord(p, tile).img * p.pack_stride;
+          const int img = tile_coord(p, tile).img;
+          const uint8_t *pack = p.pack + (long long)img * p.pack_stride;
+          if (BIAS && loaded_img != img) {
+              // bias table of this image's pack -> shared memory (this warpgroup is its only reader)
+              const float *packB = reinterpret_cast<const float *>(pack + biasOff<MODE>(PARTS));
+              tc05::named_sync(3, 128);
+              for (int i = t; i < Net<MODE>::NBIAS; i += 128) sBias[i] = __ldg(packB + i);
+              tc05::named_sync(3, 128);
+              loaded_img = img;
+          }
           for (int s = 0; s < SL; s++, n++) {
               if (ESTOP && s >= 2 && s >= sStop[it & 1]) break;
               // weight loads (thread 0): the stages of a step are, per layer, (row block, 32-column block, slab group); the next
@@ -875,6 +884,15 @@ mlp_kernel(const Params p)
                           for (int i = 0; i < 16; i++) sum[i] = sg == 0 ? d[i] : __fadd_rn(sum[i], d[i]);
 #ifndef SDB_AB_NO_ACC
                           if (sg == nsg - 1) {
+                              if (BIAS && l > 0) {
+                                  const float *b = sBias + (l - 1) * kHidden + cc * 32;
+#pragma unroll
+                                  for (int i = 0; i < 16; i += 2) {
+                                      const float2 bb = *reinterpret_cast<const float2 *>(b + tc05::frag_col(t, i));
+                                      sum[i] = __fadd_rn(sum[i], bb.x);
+                                      sum[i + 1] = __fadd_rn(sum[i + 1], bb.y);
+                                  }
+                              }
 #pragma unroll
                               for (int i = 0; i < 16; i += 2)
                                   *reinterpret_cast<float2 *>(dst + (size_t)tc05::frag_row(t, i) * kHidden + cc * 32 + tc05::frag_col(t, i)) =
@@ -1303,10 +1321,25 @@ preblend_kernel(const float *__restrict__ table, float *__restrict__ table3, int
 }
 
 // ---- weight packer ---------------------------------------------------------------------------------
-// One thread per (layer, n, k) element of the K-extended weight matrices.
+// fp32 value of the 16-bit part(s) the pack stores for v: hi (+ lo = v - hi at precision 1 / 2).  hi + lo is exact in fp32
+// (lo holds the bits below hi's), so it is what the tensor core sums for 1 * hi + 0 * hi + 1 * lo.
+template <int PREC>
+__device__ __forceinline__ float packed_value(float v) {
+    if constexpr (PREC == 1) {
+        const float hi = __bfloat162float(__float2bfloat16_rn(v));
+        return __fadd_rn(hi, __bfloat162float(__float2bfloat16_rn(v - hi)));
+    } else if constexpr (PREC == 2) {
+        const float hi = __half2float(__float2half_rn(v));
+        return __fadd_rn(hi, __half2float(__float2half_rn(v - hi)));
+    } else {
+        return __half2float(__float2half_rn(v));
+    }
+}
+
+// One thread per (layer, n, k) element of the weight matrices, then one per fp32 entry (sigma head, bias table).
 //   render: layer 0 [256 x 144]: cols 0..127 fc_1.weight, 128+lab emb[lab][n], 143 fc_1.bias;
-//           layers 1..5 [256 x 272]: cols 0..255 W*alpha, 256 beta; colour [64 x 272]: W, 256 bias
-//   sky:    layer 0 [256 x 48]: cols 0..32 fc1.weight, 47 bias (fc1.bias + fc_z_a(z)); layers 1..4, colour as above
+//           layers 1..5 [256 x 256]: W*alpha; colour [64 x 256]: W; bias table: beta of fc_2..fc_6, fc_out_c.bias
+//   sky:    layer 0 [256 x 48]: cols 0..32 fc1.weight, 47 bias (fc1.bias + fc_z_a(z)); layers 1..4, colour, bias table as above
 template <int PREC, bool SKY>
 __global__ void __launch_bounds__(256)
 pack_kernel(const float *w0, const float *b0, const float *emb, int n_labels, const float *wh, const float *bh,
@@ -1336,11 +1369,9 @@ pack_kernel(const float *w0, const float *b0, const float *emb, int n_labels, co
                 else if (k - kFeat < n_labels) v = emb[(long long)(k - kFeat) * kHidden + nn];
             }
         } else if (l == NL - 1) {
-            if (k < kHidden) v = wout[(long long)nn * kHidden + k];
-            else if (k == kHidden) v = bout[nn];
+            v = wout[(long long)nn * kHidden + k];
         } else {
-            if (k < kHidden) v = wh[((long long)(l - 1) * kHidden + nn) * kHidden + k];
-            else if (k == kHidden) v = bh[(long long)(l - 1) * kHidden + nn];
+            v = wh[((long long)(l - 1) * kHidden + nn) * kHidden + k];
         }
         uint8_t *base = pack + layerOff<MODE>(l, PARTS);
         const int nK = K / 16;
@@ -1359,14 +1390,22 @@ pack_kernel(const float *w0, const float *b0, const float *emb, int n_labels, co
         }
         return;
     }
-    if (SKY) return;
-    const long long u = t - nW;
-    if (u >= kFTotal) return;
-    float *F = reinterpret_cast<float *>(pack + layerOff<MODE>(NL, PARTS));
-    float v = 0.0f;
-    if (u < kHidden) v = wsig[u];
-    else if (u == kFBsig) v = bsig[0];
-    F[u] = v;
+    long long u = t - nW;
+    if (!SKY) {
+        if (u < kFTotal) {
+            float *F = reinterpret_cast<float *>(pack + layerOff<MODE>(NL, PARTS));
+            float v = 0.0f;
+            if (u < kHidden) v = wsig[u];
+            else if (u == kFBsig) v = bsig[0];
+            F[u] = v;
+            return;
+        }
+        u -= kFTotal;
+    }
+    if (u >= Net<MODE>::NBIAS) return;
+    const int l = 1 + (int)(u / kHidden), nn = (int)(u % kHidden);
+    const float v = l == NL - 1 ? bout[nn] : bh[(long long)(l - 1) * kHidden + nn];
+    reinterpret_cast<float *>(pack + biasOff<MODE>(PARTS))[u] = packed_value<PREC>(v);
 }
 
 template <bool SKY>
@@ -1374,7 +1413,7 @@ int launch_pack(const float *w0, const float *b0, const float *emb, int n_labels
                 const float *wsig, const float *bsig, const float *wout, const float *bout, int precision, void *pack,
                 cudaStream_t st) {
     constexpr int MODE = SKY ? kSky : kRender;
-    long long n = SKY ? 0 : kFTotal;
+    long long n = (SKY ? 0 : kFTotal) + Net<MODE>::NBIAS;
     for (int l = 0; l < Net<MODE>::NL; l++) n += (long long)layerK<MODE>(l) * layerN<MODE>(l);
     const int blocks = (int)((n + 255) / 256);
     if (precision == 1)

@@ -11,8 +11,7 @@ namespace rf {
 
 constexpr int kRows = 128, kTileW = 16, kTileH = 8;
 constexpr int kHidden = 256, kFeat = 128, kOutC = 64, kLevels = 16;
-constexpr int kKExt = 16;                       // extra K columns: labels / bias
-constexpr int kKH = kHidden + kKExt;            // 272: K of every forward layer fed by hidden activations
+constexpr int kKExt = 16;                       // extra K columns of the render network's layer 0: labels / fc_1 bias
 constexpr int kMaxM = 8, kMaxS = 64, kMaxLabels = 15;
 constexpr int kEpiThreads = 256, kGatherThreads = 256;
 // warpgroup-aligned roles so that setmaxnreg can move registers from the control group to the gather group:
@@ -28,8 +27,8 @@ static_assert(8 * 32 * kRegsLaunch + 4 * 32 * kRegsCtl + 8 * 32 * kRegsGather <=
               "setmaxnreg budget exceeds the CTA's launch-time register allocation");
 constexpr int kRingBytes = 65536;
 constexpr uint32_t kLboA = kRows * 16, kSbo = 128;
-constexpr int kHChunks = kKH / 8;               // 34 16-byte k-chunks per row
-constexpr int kHBytes = kHChunks * kRows * 16;  // 69,632 bytes per operand part
+constexpr int kHChunks = kHidden / 8;           // 32 16-byte k-chunks per row
+constexpr int kHBytes = kHChunks * kRows * 16;  // 65,536 bytes per operand part
 constexpr int kSkyK0 = 48;                      // PE(raydir) 33 + zeros + bias column 47
 constexpr int kRenderK0 = kFeat + kKExt;        // 144
 
@@ -37,7 +36,7 @@ constexpr int kRenderK0 = kFeat + kKExt;        // 144
 //   kRender: LightningMLP forward, 6 hidden layers + colour head (layers.py:92-126)
 //   kSky   : SKYMLP forward, 5 hidden layers + colour head (gancraft_base.py:150-169)
 //   kBwd   : data-gradient chain of LightningMLP: dC -> dA6 -> ... -> dA1 -> d(features); the B operands are
-//            the TRANSPOSED forward weights, there is no K extension (biases do not enter the data gradient)
+//            the TRANSPOSED forward weights (biases do not enter the data gradient)
 //   kSkyBwd: data-gradient chain of SKYMLP: dSky -> dA5 -> ... -> dA1 (the PE input needs no gradient), so there are
 //            4 operand-producing layers and the last layer's output (dA1 -> dZ1, N = 256) only goes to the record
 constexpr int kRender = 0, kSky = 1, kBwd = 2, kSkyBwd = 3;
@@ -46,13 +45,14 @@ template <int MODE> struct Net {
     static constexpr int NH = MODE == kSky ? 5 : (MODE == kSkyBwd ? 4 : 6);   // layers whose epilogue feeds the next layer
     static constexpr int NL = NH + 1;
     static constexpr int K0 = MODE == kSky ? kSkyK0 : (ISBWD ? kOutC : kRenderK0);
-    static constexpr bool EXT = !ISBWD;                     // hidden operands carry the 16-column K extension
-    static constexpr int KH = EXT ? kKH : kHidden;          // K of the layers fed by hidden activations
     static constexpr int NOUT = MODE == kBwd ? kFeat : (MODE == kSkyBwd ? kHidden : kOutC);   // N of the last layer
     static constexpr int NACT = MODE == kSky || MODE == kSkyBwd ? 5 : 6;   // hidden activations of the forward network
-    static constexpr bool TAIL = MODE == kRender || MODE == kBwd;          // the pack ends with the fp32 sigma head
+    static constexpr bool TAIL = MODE == kRender || MODE == kBwd;          // the pack has the fp32 sigma head
+    // fp32 biases of layers 1 .. NL-1 (forward networks), added to the accumulators at the write-out: entry (l - 1) * 256 + n
+    static constexpr int NBIAS = ISBWD ? 0 : (NL - 2) * kHidden + NOUT;
 };
-template <int MODE> __host__ __device__ constexpr int layerK(int l) { return l == 0 ? Net<MODE>::K0 : Net<MODE>::KH; }
+// layers fed by hidden activations have K = 256; layer 0 carries its bias (and the label embedding) in K-extension columns
+template <int MODE> __host__ __device__ constexpr int layerK(int l) { return l == 0 ? Net<MODE>::K0 : kHidden; }
 template <int MODE> __host__ __device__ constexpr int layerN(int l) { return l == Net<MODE>::NL - 1 ? Net<MODE>::NOUT : kHidden; }
 template <int MODE> __host__ __device__ constexpr int64_t layerOff(int l, int parts) {
     int64_t o = 0;
@@ -61,8 +61,12 @@ template <int MODE> __host__ __device__ constexpr int64_t layerOff(int l, int pa
 }
 // fp32 tail of the render / backward packs: sigma head
 constexpr int kFWsig = 0, kFBsig = 256, kFTotal = 264;
-template <int MODE> __host__ __device__ constexpr int64_t packBytes(int parts) {
+// the pack: the 16-bit layers, then the sigma head (TAIL), then the bias table (NBIAS floats, the last bytes of the pack)
+template <int MODE> __host__ __device__ constexpr int64_t biasOff(int parts) {
     return layerOff<MODE>(Net<MODE>::NL, parts) + (Net<MODE>::TAIL ? (int64_t)kFTotal * 4 : 0);
+}
+template <int MODE> __host__ __device__ constexpr int64_t packBytes(int parts) {
+    return biasOff<MODE>(parts) + (int64_t)Net<MODE>::NBIAS * 4;
 }
 // Byte offset of weight element (output n, input k), 16-bit part `part` (hi / lo), inside one layer of the pack, for a layer
 // of nK k16 slabs and `parts` parts.  The layer is stored in the order the MMA warpgroup streams it:
@@ -81,7 +85,7 @@ __device__ __forceinline__ bool elect_one() {
 
 // ---- shared memory map ---------------------------------------------------------------------------
 struct Smem {
-    uint32_t h_hi, h_lo, ring, fsec, scales, frac, sig, state, bars, stop, sched, total;
+    uint32_t h_hi, h_lo, ring, fsec, bias, scales, frac, sig, state, bars, stop, sched, total;
 };
 __host__ __device__ constexpr Smem smem_map(bool x3) {
     Smem m{};
@@ -90,6 +94,7 @@ __host__ __device__ constexpr Smem smem_map(bool x3) {
     m.h_lo = o; if (x3) o += kHBytes;
     m.ring = o; o += kRingBytes;
     m.fsec = o; o += kFTotal * 4;
+    m.bias = o; o += Net<kRender>::NBIAS * 4;   // the largest bias table (read by the MMA warpgroup)
     m.scales = o; o += kLevels * 4;
     m.frac = o; o += ((kMaxS + 1) * 4 + 15) / 16 * 16;
     m.sig = o; o += 2 * kRows * 4;
