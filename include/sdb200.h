@@ -491,6 +491,16 @@ int sdb_world_build(const int32_t *d_hq, const int32_t *d_label, int32_t X, int3
                     int32_t *d_world, int64_t *d_heightmap, int32_t *d_minmax, void *stream);
 int sdb_world_truncate(const int32_t *d_world, int32_t X, int32_t Z, int32_t gnd, int32_t sky, int32_t *d_voxel_t, void *stream);
 
+/* A scene of the PCG cache (the per-iteration scene switch of training, PCGCache.sample_world,
+ * imaginaire/model_utils/pcg_gen.py:26-46) scattered straight into its truncated volume.
+ *   d_sparse: the file's voxel_sparse.npy, int16 [4, nnz] row-major: rows x (height), y, z, value;
+ *   d_voxel_t int32 [sky - gnd, X, Z] is zeroed, then value is written at [x - gnd, y, z] for every entry
+ *   with gnd <= x < sky (the reference's voxel_t[gnd:sky] slice drops the others).  An entry outside
+ *   [0,SH) x [0,X) x [0,Z) is skipped.  Duplicate coordinates: any one of their values (like index_put).
+ *   Requires 0 <= gnd < sky <= SH (the caller normalises the slice), nnz >= 0.                       */
+int sdb_scene_scatter(const int16_t *d_sparse, int64_t nnz, int32_t SH, int32_t X, int32_t Z, int32_t gnd, int32_t sky,
+                      int32_t *d_voxel_t, void *stream);
+
 /* Kernels this library has launched in this process so far (every launch is counted; memsets and
  * library GEMMs are not).  bench.py reads it around its timed region for `gpu_launches`.          */
 int64_t sdb_launch_count(void);

@@ -87,6 +87,7 @@ SIGNATURES = {
     'sdb_world_build': (c_int, [c_void_p, c_void_p, c_i32, c_i32, c_i32, c_void_p, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                 c_void_p, c_void_p]),
     'sdb_world_truncate': (c_int, [c_void_p, c_i32, c_i32, c_i32, c_i32, c_void_p, c_void_p]),
+    'sdb_scene_scatter': (c_int, [c_void_p, c_i64, c_i32, c_i32, c_i32, c_i32, c_i32, c_void_p, c_void_p]),
     'sdb_launch_count': (c_i64, []),
     'sdb_debug_train_layout': (c_int, [c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, ctypes.POINTER(c_i64)]),
     'sdb_cnn_debug_record_layout': (c_int, [c_i32, c_i32, ctypes.POINTER(c_i64)]),

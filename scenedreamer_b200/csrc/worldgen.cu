@@ -13,6 +13,8 @@
 //   heightmap_kernel one thread per column scans down from the top; block-level min / max -> gnd, sky;
 //   truncate_kernel  copies world[gnd:sky] into the caller's tensor, decoding tree keys to block ids on the way.
 // Bound: HBM (one memset, one sweep for the height map, one for the copy).
+// f5 (sdb_scene_scatter): a cached world's sparse voxel list (PCGCache.sample_world, pcg_gen.py:26-46) scattered straight
+// into the truncated volume -- one memset of [sky - gnd, X, Z] and one pass over the entries.
 #include "common.cuh"
 
 namespace {
@@ -96,6 +98,22 @@ truncate_kernel(const int32_t *__restrict__ world, int32_t *__restrict__ out, lo
         out[i] = v >= (1 << kTreeShift) ? (v & ((1 << kTreeShift) - 1)) : v;
     }
 }
+
+// A cached scene's sparse voxel list ([4, nnz] int16 rows x (height), y, z, value) straight into the truncated volume
+// [sky - gnd, X, Z] (zeroed by a memset before): grid-stride over entries, each of the four rows read coalesced.  An entry
+// outside [0,SH) x [0,X) x [0,Z) is skipped (the host validates the file first), one outside [gnd, sky) is what the
+// reference's voxel_t[gnd:sky] slice drops.  Duplicate coordinates race exactly as in the reference's index_put.
+__global__ void __launch_bounds__(256)
+scene_scatter_kernel(const int16_t *__restrict__ sp, long long nnz, int SH, int X, int Z, int gnd, int sky,
+                     int32_t *__restrict__ out)
+{
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < nnz; i += stride) {
+        const int x = sp[i], y = sp[nnz + i], z = sp[2 * nnz + i];
+        if (x < 0 || x >= SH || y < 0 || y >= X || z < 0 || z >= Z || x < gnd || x >= sky) continue;
+        out[((long long)(x - gnd) * X + y) * Z + z] = (int32_t)sp[3 * nnz + i];
+    }
+}
 }  // namespace
 
 // Stage 1: fills d_world [SH, X, Z] (caller-owned scratch), the height map [X, Z] (int64, like the reference's) and
@@ -133,6 +151,21 @@ extern "C" int sdb_world_truncate(const int32_t *d_world, int32_t X, int32_t Z, 
     const long long plane = (long long)X * Z, n = plane * (sky - gnd);
     const long long want = (n + 255) / 256, cap = (long long)sdb_num_sms() * 32;
     truncate_kernel<<<(int)(want < cap ? want : cap), 256, 0, (cudaStream_t)stream>>>(d_world, d_voxel_t, n, plane * gnd);
+    SDB_CHECK_LAUNCH();
+    return SDB_OK;
+}
+
+// A scene of the PCG cache: d_voxel_t [sky - gnd, X, Z] = zeros, then value at [x - gnd, y, z] for every entry of d_sparse
+// ([4, nnz] int16) with gnd <= x < sky.  gnd / sky are the caller's normalised slice bounds of range(SH).
+extern "C" int sdb_scene_scatter(const int16_t *d_sparse, int64_t nnz, int32_t SH, int32_t X, int32_t Z, int32_t gnd, int32_t sky,
+                                 int32_t *d_voxel_t, void *stream)
+{
+    if (!d_sparse || !d_voxel_t || nnz < 0 || SH <= 0 || X <= 0 || Z <= 0 || !(0 <= gnd && gnd < sky && sky <= SH)) return SDB_EINVAL;
+    cudaStream_t st = (cudaStream_t)stream;
+    SDB_CUDA(cudaMemsetAsync(d_voxel_t, 0, (size_t)X * Z * (sky - gnd) * 4, st));
+    if (nnz == 0) return SDB_OK;
+    const long long want = (nnz + 255) / 256, cap = (long long)sdb_num_sms() * 16;
+    scene_scatter_kernel<<<(int)(want < cap ? want : cap), 256, 0, st>>>(d_sparse, nnz, SH, X, Z, gnd, sky, d_voxel_t);
     SDB_CHECK_LAUNCH();
     return SDB_OK;
 }

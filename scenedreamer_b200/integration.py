@@ -576,6 +576,9 @@ def ensure_installed():
             pcg = sys.modules.get('imaginaire.model_utils.pcg_gen')
             if pcg is not None and hasattr(pcg, 'PCGVoxelGenerator') and os.environ.get('SDB200_WORLDGEN', '1') != '0':
                 worldgen.install(pcg.PCGVoxelGenerator)             # f3: the scene's voxel world is built on the device
+            if pcg is not None and hasattr(pcg, 'PCGCache'):
+                worldgen.install(pcg.PCGCache)                      # f5: cached scenes read ahead, scattered on the device
+                                                                    # (SDB200_SCENECACHE=0 is read per call)
         _installed = True
 
 

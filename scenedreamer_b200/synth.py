@@ -182,3 +182,43 @@ def frame_camera(world, pose, resolution_hw=(540, 960), pad=30):
     f = cam_f * (resolution_hw[1] - 1)
     c = [(cam_res[0] - 1) / 2, (cam_res[1] - 1) / 2]
     return cam_ori, cam_dir, cam_up, float(f), c, cam_res
+
+
+def write_cache_world(d, size=1024, seed=3407, shell=9, peak=False, bad=None):
+    """A world of the PCG scene cache in the layout scripts/pcg_cache.py writes (what PCGCache.sample_world reads):
+    voxel_sparse.npy int16 [4, nnz] (rows height, x, z, block id, in np.where order), height_map.npy float32 [1,1,X,Z],
+    semantic_map.npy float32 [1,11,X,Z] (one-hot, 10 = tree), hmap_mc.npy int64 [X,Z] (topmost occupied height).
+    Seeded terrain (make_bev): a `shell`-voxel surface shell per column plus a trunk / canopy column at the tree cells
+    (9 voxels per column and ~1 % trees: about 9.5 M entries at 1024^2).  peak: one column reaches the top layer (sky 256).
+    bad = (row, value): the first entry's coordinate in that row replaced (a malformed file)."""
+    import os
+    h, sem, tree = make_bev(size, seed)
+    h = h.copy()
+    h[h < 0] = 0
+    hq = ((h - h.min()) / (1 - h.min()) * (SAMPLE_HEIGHT - 1)).astype(np.int64)
+    has_tree = tree != 255
+    tlen = np.where(has_tree, 6 + (np.arange(size * size).reshape(size, size) % 7), 0)
+    if peak:
+        hq[size // 2, size // 3] = SAMPLE_HEIGHT - shell
+        tlen[size // 2, size // 3] = 0
+    surf = hq + shell - 1
+    top = np.minimum(surf + tlen, SAMPLE_HEIGHT - 1)
+    label = BIOME2MC[sem.astype(np.int64)]
+    rows = []
+    for x in range(int(hq.min()), int(top.max()) + 1):
+        ys, zs = np.nonzero((hq <= x) & (x <= top))
+        v = np.where(x <= surf[ys, zs], label[ys, zs], np.where(x > top[ys, zs] - 4, 18, 17))
+        rows.append(np.stack([np.full(ys.shape, x), ys, zs, v]))
+    sparse = np.concatenate(rows, 1).astype(np.int16)
+    if bad is not None:
+        sparse[bad[0], 0] = bad[1]
+    org = sem.astype(np.int64)
+    org[has_tree] = 10
+    onehot = np.zeros((1, 11, size, size), np.float32)
+    np.put_along_axis(onehot[0], org[None], 1.0, axis=0)
+    os.makedirs(d, exist_ok=True)
+    np.save(os.path.join(d, 'voxel_sparse.npy'), sparse)
+    np.save(os.path.join(d, 'height_map.npy'), (surf / (SAMPLE_HEIGHT - 1)).astype(np.float32)[None, None])
+    np.save(os.path.join(d, 'semantic_map.npy'), onehot)
+    np.save(os.path.join(d, 'hmap_mc.npy'), top.astype(np.int64))
+    return d
