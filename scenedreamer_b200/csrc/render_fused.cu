@@ -17,7 +17,7 @@
 //     so compositing is a per-thread running sum (no cross-thread reduction, any S);
 //   * warp roles: 8 epilogue warps (accumulator row -> LeakyReLU -> 16-bit operand in smem; sigma tap;
 //     compositing; warps 0-3 own columns 0..127, warps 4-7 columns 128..255 of the same 128 rows),
-//     one MMA warpgroup (wgmma in 64x32 blocks; its thread 0 also streams the weights into a 4-slot ring
+//     one MMA warpgroup (wgmma in 64x64 blocks; its thread 0 also streams the weights into a 4-slot ring
 //     with 1-D bulk TMA copies), 8 gather warps (hash-grid fetch for the NEXT sample step while the MLP
 //     of the current one runs; results wait in registers until the operand buffer is free);
 //   * accumulators: a layer's fp32 [128 x 256] result (128 KB) fits neither next to the operand buffers in
@@ -447,6 +447,7 @@ mlp_kernel(const Params p)
     const uint32_t mask = SKY ? 0u : ((1u << p.log2_T) - 1u);
 
     if (warp < 8) {
+        set_maxnreg<kRegsEpi>();
         // =========================== EPILOGUE / COMPOSITING WARPS ===========================
         const int row = tid & (kRows - 1), half = tid >> 7;          // column half: 128*half .. +127
         // 64-row block of this thread (warps 0,1,4,5 / 2,3,6,7): its hand-offs with the MMA warpgroup and its compositing
@@ -780,23 +781,29 @@ mlp_kernel(const Params p)
             }
         }
     } else if (warp < kGatherWarp0) {
-      asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegsCtl));
+      set_maxnreg<kRegsCtl>();
       // =========================== MMA WARPGROUP ===========================
-      // Layer l of a sample step: D[128 x N] = H[128 x K] * W_l^T, one 64-row block rb after the other, each in 32-column
+      // Layer l of a sample step: D[128 x N] = H[128 x K] * W_l^T, one 64-row block rb after the other, each in 64-column
       // blocks (the sum over K in registers) written once to this CTA's fp32 accumulator buffer (g & 1) in global memory, where
       // the epilogue reads its rows.  A row block is handed over as soon as it is written, so the epilogue of one row block runs
-      // while the MMAs of the other do.  Weights go through a 4-slot ring of 16 KB stages = up to 8 k16 slabs of one 32-column
-      // block, one bulk copy each (wpack_off); thread 0 keeps the ring full, the weights are streamed once per row block.
-      // Named barrier 3 is this warpgroup's (1, 4, 5: epilogue, 2: gather).
+      // while the MMAs of the other do.  Weights go through a 4-slot ring of 16 KB stages (4 k16 slabs of one 64-column block
+      // at x3, 8 at x1; a hidden-layer block at x3 fills the whole ring), one bulk copy each (wpack_off); thread 0 keeps the
+      // ring full, the weights are streamed once per row block.  Named barrier 3 is this warpgroup's (1, 4, 5: epilogue,
+      // 2: gather).
       //
-      // Numerics: every stage starts a fresh tensor-core sum that is added to the block's running sum in fp32 with round-to-
-      // nearest, in stage order: the tensor core's own accumulation does not round to nearest, and over a whole x3 layer (up to
-      // 51 chained MMAs) that moved the full-frame depth outside its parity bound.  Two accumulator sets alternate, so that the
-      // add and the ring-slot release of one stage overlap the MMAs of the next.  Layers 1 .. NL-1 of the forward networks
+      // Numerics: slabs 0..7 of a block and slabs 8..nK-1 are two fresh tensor-core sums d0, d1 (numerics groups), and the
+      // block is RN(d0 + d1), or d0 when nK <= 8: the tensor core's own accumulation does not round to nearest, and over a
+      // whole x3 layer that moved the full-frame depth outside its parity bound.  Layers 1 .. NL-1 of the forward networks
       // then add their fp32 bias (the pack's table: hi + lo of the 16-bit parts, what a bias K slab would have summed on the
-      // tensor core, exactly) with one more round-to-nearest add, so a hidden 32-column block is exactly two full stages.
+      // tensor core, exactly) with one more round-to-nearest add.  Two 32-register sets X, Y alternate: block c's group 0 is
+      // in X, its group 1 goes to Y; once both are done X = RN(RN(X + Y) + b), block c + 1's group 0 is issued into Y and X is
+      // stored while it runs, then block c + 1's group 1 goes to X, and so on.  Every stage is its own commit group, so its
+      // ring slot is released (and refilled with a stage of the next block) as soon as its MMAs are done.
       const int t = tid - kMmaWarp0 * 32;
-      constexpr uint32_t kSlot = 16384, kSlabB = 1024 * PARTS;       // ring slot; one k16 slab of a 32-column block
+      constexpr uint32_t kSlot = 16384, kSlabB = 2048 * PARTS;       // ring slot; one k16 slab of a 64-column block
+      constexpr int kSps = kSlot / kSlabB;                           // slabs per ring slot
+      static_assert(block_stages(kHidden / 16, kSps) <= 4 && block_stages(kRenderK0 / 16, kSps) <= 4,
+                    "the stages of one column block fit the 4-slot ring");
       constexpr bool BIAS = Net<MODE>::NBIAS > 0;
       uint32_t n = 0, q = 0, qr = 0;                                 // ring stages issued to the tensor cores / retired
       int loaded_img = -1;
@@ -816,26 +823,32 @@ mlp_kernel(const Params p)
           }
           for (int s = 0; s < SL; s++, n++) {
               if (ESTOP && s >= 2 && s >= sStop[it & 1]) break;
-              // weight loads (thread 0): the stages of a step are, per layer, (row block, 32-column block, slab group); the next
-              // one to load is stage pj of layer pl, ring index pq
-              int pl = 0, pj = 0;
-              uint32_t pq = q;
+              // weight loads (thread 0): the stages of a step are, per layer and row block, the layer's bytes in pack order (the
+              // pack is stored in streaming order, wpack_off), cut at stage boundaries.  The next one to load is stage js of a
+              // block of layer pl, row block pr, at byte po of the pack, ring index pq.
+              int pl = 0, pr = 0, js = 0;
+              uint32_t pq = q, po = 0;
               auto produce = [&](uint32_t upto) {
                   for (; pq < upto && pl < NL; pq++) {
-                      const int nK = layerK<MODE>(pl) / 16, nsg = (nK + 7) / 8, per_rb = layerN<MODE>(pl) / 32 * nsg;
-                      const int j = pj < per_rb ? pj : pj - per_rb, cc = j / nsg, kk0 = (j - cc * nsg) * 8;
-                      const uint32_t bytes = (uint32_t)min(8, nK - kk0) * kSlabB, slot = pq & 3u;
+                      const int nK = layerK<MODE>(pl) / 16;
+                      const uint32_t bytes = (uint32_t)stage_slabs(nK, kSps, js) * kSlabB, slot = pq & 3u;
                       tc05::mbar_arrive_expect_tx(&bars[B_WFULL + slot], bytes);
-                      tc05::bulk_g2s(sRing + slot * kSlot, pack + layerOff<MODE>(pl, PARTS) + wpack_off(nK, PARTS, cc * 32, kk0 * 16, 0),
-                                     bytes, &bars[B_WFULL + slot]);
-                      if (++pj == 2 * per_rb) { pj = 0; pl++; }
+                      tc05::bulk_g2s(sRing + slot * kSlot, pack + po, bytes, &bars[B_WFULL + slot]);
+                      po += bytes;
+                      if (++js == block_stages(nK, kSps)) js = 0;
+                      if (po == (uint32_t)layerOff<MODE>(pl + 1, PARTS)) {       // end of the layer: again for row block 1, or the next layer
+                          if (pr == 0) po = (uint32_t)layerOff<MODE>(pl, PARTS);
+                          else pl++;
+                          pr ^= 1;
+                      }
                   }
               };
               if (t == 0) produce(q + 4);
 #pragma unroll 1
               for (int l = 0; l < NL; l++) {
                   const uint32_t g = n * NL + l, buf = g & 1u;
-                  const int N = layerN<MODE>(l), nK = layerK<MODE>(l) / 16, nsg = (nK + 7) / 8, nst = N / 32 * nsg;
+                  const int N = layerN<MODE>(l), nK = layerK<MODE>(l) / 16;
+                  const int ncb = N / 64, nsb = block_stages(nK, kSps), ns0 = group0_stages(nK, kSps);
 #pragma unroll 1
                   for (int rb = 0; rb < 2; rb++) {
                       if (t == 0) SDB_MARK(2, 1, n, l);
@@ -848,75 +861,98 @@ mlp_kernel(const Params p)
                       }
                       if (t == 0) SDB_MARK(2, 2, n, l);
                       if (t == 0) SDB_STAMP(n, l, 2 * rb);
-                      float *dst = p.acc + (((size_t)blockIdx.x * 2 + buf) * kRows + rb * 64) * kHidden;
-                      float da[16], db[16], sum[16];
-                      // stage j of this row block (32-column block j / nsg, slab group j % nsg): issue its MMAs into d
-                      auto mma = [&](float (&d)[16], int j) {
-                          const uint32_t slot = q & 3u;
-                          tc05::mbar_wait(&bars[B_WFULL + slot], (q >> 2) & 1u);
-                          const uint32_t sb = tc05::smem_u32(sRing + slot * kSlot);
-                          const int kk0 = (j % nsg) * 8, ns = min(8, nK - kk0);
-                          tc05::wgmma_fence();
+                      TSplit ts;
+                      ts.start();
+                      // element offset of these rows in the accumulator buffers (p.acc is re-read at the store: a 64-bit pointer
+                      // held across the block loop would not fit the registers next to the two accumulator sets)
+                      const uint32_t dst = ((blockIdx.x * 2 + buf) * kRows + rb * 64) * kHidden;
+                      float x[32], y[32];
+                      // issue the MMAs of stages [js0, js1) of the current block into d, one commit group per stage; the first
+                      // slab of stage js0 starts a fresh sum (js0 = the first stage of a numerics group)
+                      auto issue = [&](float (&d)[32], int js0, int js1) {
+                          for (int js = js0; js < js1; js++) {
+                              const uint32_t slot = q & 3u;
+                              tc05::mbar_wait(&bars[B_WFULL + slot], (q >> 2) & 1u);
+                              ts.lap(kSplitFull);
+                              const uint32_t sb = tc05::smem_u32(sRing + slot * kSlot);
+                              const int kk0 = stage_slab0(nK, kSps, js), ns = stage_slabs(nK, kSps, js);
+                              tc05::wgmma_fence();
 #pragma unroll
-                          for (int i = 0; i < 8; i++) {
-                              if (i >= ns) break;
-                              const uint32_t aoff = (uint32_t)(kk0 + i) * 2 * kLboA + rb * 1024;
-                              const uint64_t ah = tc05::make_smem_desc(tc05::smem_u32(sHhi) + aoff, kLboA, kSbo);
-                              const uint64_t bh = tc05::make_smem_desc(sb + i * kSlabB, 512, kSbo);
-                              tc05::wgmma_m64n32k16<BF16, 0, 0>(d, ah, bh, i > 0 ? 1u : 0u);
-                              if constexpr (X3) {
-                                  const uint64_t al = tc05::make_smem_desc(tc05::smem_u32(sHlo) + aoff, kLboA, kSbo);
-                                  tc05::wgmma_m64n32k16<BF16, 0, 0>(d, al, bh, 1u);
-                                  tc05::wgmma_m64n32k16<BF16, 0, 0>(d, ah, bh + (1024 >> 4), 1u);
-                              }
-                          }
-                          tc05::wgmma_commit();
-                          q++;
-                      };
-                      // the MMAs of stage j (in d) are complete: refill its ring slot, add its sum, store a finished block
-                      auto retire = [&](float (&d)[16], int j) {
-                          tc05::wgmma_fence_acc(d);
-                          tc05::named_sync(3, 128);           // every warp is done with the slot
-                          if (t == 0) produce(qr + 5);
-                          qr++;
-                          const int cc = j / nsg, sg = j - cc * nsg;
-#pragma unroll
-                          for (int i = 0; i < 16; i++) sum[i] = sg == 0 ? d[i] : __fadd_rn(sum[i], d[i]);
-#ifndef SDB_AB_NO_ACC
-                          if (sg == nsg - 1) {
-                              if (BIAS && l > 0) {
-                                  const float *b = sBias + (l - 1) * kHidden + cc * 32;
-#pragma unroll
-                                  for (int i = 0; i < 16; i += 2) {
-                                      const float2 bb = *reinterpret_cast<const float2 *>(b + tc05::frag_col(t, i));
-                                      sum[i] = __fadd_rn(sum[i], bb.x);
-                                      sum[i + 1] = __fadd_rn(sum[i + 1], bb.y);
+                              for (int i = 0; i < kSps; i++) {
+                                  if (i >= ns) break;
+                                  const uint32_t aoff = (uint32_t)(kk0 + i) * 2 * kLboA + rb * 1024;
+                                  const uint64_t ah = tc05::make_smem_desc(tc05::smem_u32(sHhi) + aoff, kLboA, kSbo);
+                                  const uint64_t bh = tc05::make_smem_desc(sb + i * kSlabB, 1024, kSbo);
+                                  tc05::wgmma_m64n64k16<BF16, 0, 0>(d, ah, bh, (js > js0 || i > 0) ? 1u : 0u);
+                                  if constexpr (X3) {
+                                      const uint64_t al = tc05::make_smem_desc(tc05::smem_u32(sHlo) + aoff, kLboA, kSbo);
+                                      tc05::wgmma_m64n64k16<BF16, 0, 0>(d, al, bh, 1u);
+                                      tc05::wgmma_m64n64k16<BF16, 0, 0>(d, ah, bh + (2048 >> 4), 1u);
                                   }
                               }
-#pragma unroll
-                              for (int i = 0; i < 16; i += 2)
-                                  *reinterpret_cast<float2 *>(dst + (size_t)tc05::frag_row(t, i) * kHidden + cc * 32 + tc05::frag_col(t, i)) =
-                                      make_float2(sum[i], sum[i + 1]);
+                              tc05::wgmma_commit();
+                              q++;
+                              ts.lap(kSplitIssue);
                           }
-#endif
                       };
-                      static_assert(kHidden % 64 == 0 && kOutC % 64 == 0 && kFeat % 64 == 0, "stages go in pairs: every N is a multiple of 64");
+                      // block c: its group 0 is in flight in a.  Issue group 1 into b, release the block's ring slots in stage
+                      // order as their MMAs complete, reduce into a, start block c + 1's group 0 in b and store a.
+                      auto block = [&](float (&a)[32], float (&b)[32], int c) {
+                          issue(b, ns0, nsb);
+                          auto release = [&]() {
+                              ts.lap(kSplitWait);
+                              tc05::named_sync(3, 128);       // every warp is done with the slot
+                              if (t == 0) produce(qr + 5);
+                              qr++;
+                              ts.lap(kSplitRetire);
+                          };
 #pragma unroll 1
-                      for (int j = 0; j < nst; j += 2) {
-                          mma(da, j);
-                          if (j > 0) {
-                              tc05::wgmma_wait<1>();
-                              retire(db, j - 1);
+                          for (int k = nsb - 1; k > 0; k--) {
+                              tc05::wgmma_wait_n(k);
+                              release();
                           }
-                          mma(db, j + 1);
-                          tc05::wgmma_wait<1>();
-                          retire(da, j);
+                          tc05::wgmma_wait<0>();
+                          release();
+                          tc05::wgmma_fence_acc(a);
+                          tc05::wgmma_fence_acc(b);
+                          if (nsb > ns0) {
+#pragma unroll
+                              for (int i = 0; i < 32; i++) a[i] = __fadd_rn(a[i], b[i]);
+                          }
+                          // the thread's fragment position, re-read here: held across the block loop it was spilled
+                          uint32_t ft;
+                          asm volatile("mov.u32 %0, %%tid.x;" : "=r"(ft));
+                          ft -= kMmaWarp0 * 32;
+                          if (BIAS && l > 0) {
+                              const float *bias = sBias + (l - 1) * kHidden + c * 64;
+#pragma unroll
+                              for (int i = 0; i < 32; i += 2) {
+                                  const float2 bb = *reinterpret_cast<const float2 *>(bias + tc05::frag_col(ft, i));
+                                  a[i] = __fadd_rn(a[i], bb.x);
+                                  a[i + 1] = __fadd_rn(a[i + 1], bb.y);
+                              }
+                          }
+                          ts.lap(kSplitRetire);
+                          if (c + 1 < ncb) issue(b, 0, ns0);
+#ifndef SDB_AB_NO_ACC
+#pragma unroll
+                          for (int i = 0; i < 32; i += 2)
+                              *reinterpret_cast<float2 *>(p.acc + (dst + (uint32_t)(tc05::frag_row(ft, i) * kHidden + c * 64 + tc05::frag_col(ft, i)))) =
+                                  make_float2(a[i], a[i + 1]);
+#endif
+                          ts.lap(kSplitRetire);
+                      };
+                      issue(x, 0, ns0);
+#pragma unroll 1
+                      for (int c = 0; c < ncb; c += 2) {
+                          block(x, y, c);
+                          if (c + 1 < ncb) block(y, x, c + 1);
                       }
-                      tc05::wgmma_wait<0>();
-                      retire(db, nst - 1);
                       __threadfence_block();
                       tc05::named_sync(3, 128);
+                      ts.lap(kSplitRetire);
                       if (t == 0) SDB_STAMP(n, l, 2 * rb + 1);
+                      if (t == 0) SDB_STAMP_SPLIT(n, l, rb, ts);
                       if (t == 0) {
                           if (l == NL - 1) {
                               tc05::mbar_arrive(&bars[B_OUTRDY + rb]);
@@ -931,7 +967,7 @@ mlp_kernel(const Params p)
       }
     } else {
         // =========================== GATHER WARPS (layer-0 operand producers) ===========================
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegsGather));
+        set_maxnreg<kRegsGather>();
         const int gt = tid - kGatherWarp0 * 32;
         const int row = gt & (kRows - 1), half = gt >> 7;
         uint32_t n = 0;

@@ -14,17 +14,23 @@ constexpr int kHidden = 256, kFeat = 128, kOutC = 64, kLevels = 16;
 constexpr int kKExt = 16;                       // extra K columns of the render network's layer 0: labels / fc_1 bias
 constexpr int kMaxM = 8, kMaxS = 64, kMaxLabels = 15;
 constexpr int kEpiThreads = 256, kGatherThreads = 256;
-// warpgroup-aligned roles so that setmaxnreg can move registers from the control group to the gather group:
+// warpgroup-aligned roles so that setmaxnreg can move registers between them (here: from the epilogue to the MMA warpgroup):
 //   WG0-1 epilogue (warps 0-7), WG2 MMA + weight loads (warps 8-11), WG3-4 gather (12-19)
 constexpr int kMmaWarp0 = 8, kGatherWarp0 = 12;
 constexpr int kThreads = kEpiThreads + 128 + kGatherThreads;   // 640
 // setmaxnreg can only redistribute the registers the CTA was LAUNCHED with (640 threads x 96 = 61,440; the
 // allocator is a per-CTA pool -- USETMAXREG.TRY_ALLOC.CTAPOOL spins forever otherwise):
-//   8 epilogue warps x 96 + 4 control warps x 80 + 8 gather warps x 104 = 61,440
-// (the MMA warpgroup holds two 16-register accumulator sets and the running sum: 48 would spill inside its stage loop)
-constexpr int kRegsLaunch = 96, kRegsCtl = 80, kRegsGather = 104;
-static_assert(8 * 32 * kRegsLaunch + 4 * 32 * kRegsCtl + 8 * 32 * kRegsGather <= kThreads * kRegsLaunch,
+//   8 epilogue warps x 80 + 4 control warps x 112 + 8 gather warps x 104 = 61,440
+// (the MMA warpgroup holds two 32-register accumulator sets of 64-column blocks and its loop state; at 96 that state spills
+// inside the stage loop)
+constexpr int kRegsLaunch = 96, kRegsEpi = 80, kRegsCtl = 112, kRegsGather = 104;
+static_assert(8 * 32 * kRegsEpi + 4 * 32 * kRegsCtl + 8 * 32 * kRegsGather <= kThreads * kRegsLaunch,
               "setmaxnreg budget exceeds the CTA's launch-time register allocation");
+// a role's register count: released to / taken from the CTA's pool (no instruction when it is the launch count)
+template <int R> __device__ __forceinline__ void set_maxnreg() {
+    if constexpr (R < kRegsLaunch) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+    else if constexpr (R > kRegsLaunch) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
+}
 constexpr int kRingBytes = 65536;
 constexpr uint32_t kLboA = kRows * 16, kSbo = 128;
 constexpr int kHChunks = kHidden / 8;           // 32 16-byte k-chunks per row
@@ -70,11 +76,27 @@ template <int MODE> __host__ __device__ constexpr int64_t packBytes(int parts) {
 }
 // Byte offset of weight element (output n, input k), 16-bit part `part` (hi / lo), inside one layer of the pack, for a layer
 // of nK k16 slabs and `parts` parts.  The layer is stored in the order the MMA warpgroup streams it:
-//   [32-column block n/32][k16 slab k/16][part][k-chunk (k/8)%2][32 outputs][8 k]
-// so one k16 slab of a 32-column block is a 1 KB-per-part wgmma B operand (K-major, no swizzle, LBO 512), and a ring stage
-// (up to 8 consecutive slabs of one block) is ONE contiguous range that a single bulk copy fetches.
+//   [64-column block n/64][k16 slab k/16][part][k-chunk (k/8)%2][64 outputs][8 k]
+// so one k16 slab of a 64-column block is a 2 KB-per-part wgmma B operand (K-major, no swizzle, LBO 1024), and a ring stage
+// (consecutive slabs of one block) is ONE contiguous range that a single bulk copy fetches.
 __host__ __device__ constexpr int64_t wpack_off(int nK, int parts, int n, int k, int part) {
-    return ((((int64_t)(n >> 5) * nK + (k >> 4)) * parts + part) * 2 + ((k >> 3) & 1)) * 512 + (n & 31) * 16 + (k & 7) * 2;
+    return ((((int64_t)(n >> 6) * nK + (k >> 4)) * parts + part) * 2 + ((k >> 3) & 1)) * 1024 + (n & 63) * 16 + (k & 7) * 2;
+}
+static_assert(kHidden % 64 == 0 && kOutC % 64 == 0 && kFeat % 64 == 0, "every layer is whole 64-column blocks");
+
+// Ring stages of one 64-column block of a layer with nK k16 slabs, `sps` slabs per ring slot.  The block's sum over K is two
+// numerics groups -- slabs 0..7 and slabs 8..nK-1, each a fresh tensor-core sum -- and a stage never straddles them.
+__host__ __device__ constexpr int group0_stages(int nK, int sps) { return ((nK < 8 ? nK : 8) + sps - 1) / sps; }
+__host__ __device__ constexpr int block_stages(int nK, int sps) {
+    return group0_stages(nK, sps) + ((nK > 8 ? nK - 8 : 0) + sps - 1) / sps;
+}
+// first slab and slab count of stage js of a block
+__host__ __device__ constexpr int stage_slab0(int nK, int sps, int js) {
+    return js < group0_stages(nK, sps) ? js * sps : 8 + (js - group0_stages(nK, sps)) * sps;
+}
+__host__ __device__ constexpr int stage_slabs(int nK, int sps, int js) {
+    const int end = js < group0_stages(nK, sps) ? (nK < 8 ? nK : 8) : nK, left = end - stage_slab0(nK, sps, js);
+    return left < sps ? left : sps;
 }
 
 __device__ __forceinline__ bool elect_one() {
@@ -224,11 +246,32 @@ __device__ __forceinline__ void acc_ld(const float *src, float (&v)[NV]) {
 //   slot 2 rb + 1  MMA warpgroup, row block rb: the accumulators are written
 //   slot 4 + 2 rb  epilogue of row block rb: accumulators seen        slot 5 + 2 rb: the next layer's operand rows handed over
 //   layer row 7 = the gather role preparing step n: 0 compositing of step n-2 seen, 1 slots refilled, 2 features gathered, 3 operand buffer free
+// and the MMA warpgroup's row-block time (slot 2 rb -> slot 2 rb + 1) split into cycles spent in kSplit* (thread 0's clock):
+//   debug[kSplitBase + ((n - first) * 8 + layer) * 8 + rb * 4 + k]
 constexpr int32_t kTraceMagic = 0x7131;
-constexpr int kTraceSteps = 6;
+constexpr int kTraceSteps = 6, kSplitBase = 512;
+enum { kSplitFull = 0, kSplitIssue, kSplitWait, kSplitRetire };   // full-barrier waits, wgmma issue, wait_group, retire / add / store
 #ifndef SDB_TIMELINE
 #define SDB_STAMP(n_, layer, slot) do { } while (0)      // compiled out: the stamps cost the epilogue role registers (spills)
+struct TSplit {
+    __device__ __forceinline__ void start() {}
+    __device__ __forceinline__ void lap(int) {}
+};
+#define SDB_STAMP_SPLIT(n_, layer, rb, ts) do { } while (0)
 #else
+struct TSplit {                                   // cycles since the last lap, charged to category k
+    uint32_t acc[4], t;
+    __device__ __forceinline__ void start() { acc[0] = acc[1] = acc[2] = acc[3] = 0; t = (uint32_t)clock(); }
+    __device__ __forceinline__ void lap(int k) { const uint32_t c = (uint32_t)clock(); acc[k] += c - t; t = c; }
+};
+#define SDB_STAMP_SPLIT(n_, layer, rb, ts)                                                                         \
+    do {                                                                                                           \
+        if (p.debug != nullptr && blockIdx.x == 0 && p.debug[60] == kTraceMagic) {                                 \
+            const int rel__ = (int)(n_) - p.debug[61];                                                             \
+            if (rel__ >= 0 && rel__ < kTraceSteps)                                                                 \
+                for (int k__ = 0; k__ < 4; k__++) p.debug[kSplitBase + (rel__ * 8 + (layer)) * 8 + (rb) * 4 + k__] = (int32_t)(ts).acc[k__]; \
+        }                                                                                                          \
+    } while (0)
 #define SDB_STAMP(n_, layer, slot)                                                                                 \
     do {                                                                                                           \
         if (p.debug != nullptr && blockIdx.x == 0 && p.debug[60] == kTraceMagic) {                                 \

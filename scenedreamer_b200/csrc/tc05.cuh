@@ -87,6 +87,15 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// the same with a warp-uniform run-time count; counts above 3 wait for at most 3 pending groups
+__device__ __forceinline__ void wgmma_wait_n(int n) {
+    switch (n) {
+    case 0: wgmma_wait<0>(); break;
+    case 1: wgmma_wait<1>(); break;
+    case 2: wgmma_wait<2>(); break;
+    default: wgmma_wait<3>(); break;
+    }
+}
 // keeps the compiler from moving accumulator reads / writes across an in-flight wgmma
 template <int R>
 __device__ __forceinline__ void wgmma_fence_acc(float (&d)[R]) {
