@@ -334,6 +334,19 @@ typedef struct sdb_render_view_grads {
 } sdb_render_view_grads;
 int sdb_render_rays_backward_views(const sdb_render_params *p, const void *d_record, const sdb_render_view_grads *g, void *stream);
 
+/* The same backward for a forward that kept NO record (sdb_render_rays_forward with early termination off, whose outputs
+ * equal the recording forward's), so that a batch needs one view's record instead of n_img.  `p` is the forward's params
+ * (n_img >= 1, pre-blended table, precision 0 or 2; raw 5-D table or precision 1 -> SDB_EUNSUPPORTED), `g` and its strides
+ * mean what they mean for sdb_render_rays_backward_views.  For each view i the call rebuilds view i's record in
+ * d_view_record (sdb_render_train_record_bytes(1, H, W, S) bytes, reused for every view) with the training prepass and the
+ * recording forward over view i alone -- its rays, uniforms, camera origin, sky, sky_avg and pack (mlp_pack_stride) -- then
+ * runs stages 1-4 for view i over it; stage 3b runs once per batch.  It writes none of the forward's outputs (d_net_out,
+ * d_weights_out, ...): the recomputed net_out goes to the backward workspace, whose size is unchanged.  Asynchronous like
+ * the record-mode backward; after the call d_view_record holds the record of the last view.  The cost over record mode is
+ * one recording forward per view.                                                                                    */
+int sdb_render_rays_backward_recompute(const sdb_render_params *p, void *d_view_record, const sdb_render_view_grads *g,
+                                       void *stream);
+
 /* --------------------------------------------------------------------------------------------
  * a9 under autograd.  sdb_sky_train_forward = sdb_sky_forward (fp16x3, ONE style code / image)
  * that also records PE(raydir), the five hidden activations (bf16) and their LeakyReLU sign

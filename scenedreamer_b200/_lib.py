@@ -66,6 +66,7 @@ SIGNATURES = {
     'sdb_sky_backward': (c_int, [c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                  c_void_p]),
     'sdb_render_rays_backward_views': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    'sdb_render_rays_backward_recompute': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
     'sdb_sky_train_forward_views': (c_int, [c_void_p, c_i32, c_i32, c_i32, c_void_p, c_i64, c_void_p, c_void_p, c_void_p, c_void_p,
                                             c_void_p]),
     'sdb_sky_backward_views': (c_int, [c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_void_p, c_void_p]),

@@ -419,16 +419,38 @@ extern "C" int sdb_render_rays_train_forward(const sdb_render_params *sp, void *
 static const int64_t kRenderGradSize[5] = {(int64_t)rf::kHidden * rf::kX0Cols, (int64_t)5 * rf::kHidden * rf::kActCols,
                                            (int64_t)8 * rf::kActCols, (int64_t)rf::kOutC * rf::kActCols, rf::kOutC};
 
-static int render_backward(const sdb_render_params *sp, const void *d_record, const sdb_render_grads *g, const int64_t *gstride,
-                           void *stream)
+// The backward of a batch in three parts, shared by the record-mode entries (every view's items in the forward's record)
+// and the recompute entry (one view's record rebuilt just before its stages): backward_begin zeroes the outputs,
+// backward_view runs stages 1-4 for one view over a record, backward_finish runs stage 3b once for the batch.
+namespace rf {
+struct BwdBatch {
+    const sdb_render_grads *g;
+    const int64_t *gstride;                  // floats between the views' gradients: w1ext, wh, wsig, wout, sky_avg
+    long long tpi, hw;                       // tiles and rays of one view
+    float *dc32, *dsig32, *dx0, *dt3;        // the one-view backward workspace
+    uint16_t *dc16, *dsig16, *dz;
+    // SDB_TIMING=1: per-stage device times on stderr, summed over the views (diagnostics; synchronises).  An event closes the
+    // interval since the previous one and charges it to its stage: 0 compositing, 1 chain, 2 table, 3 weight GEMMs, 4 table
+    // transpose (reported with the table), 5 the recompute forward
+    bool timing;
+    cudaEvent_t tev0;
+    std::vector<std::pair<int, cudaEvent_t>> tev;
+    void mark(int stage, cudaStream_t st) {
+        if (!timing) return;
+        tev.emplace_back(stage, nullptr);
+        cudaEventCreate(&tev.back().second);
+        cudaEventRecord(tev.back().second, st);
+    }
+};
+
+// argument checks of a backward (before any CUDA call); p = the forward's params
+static int backward_check(const sdb_render_params *sp, const void *d_record, const sdb_render_grads *g, const int64_t *gstride,
+                          Params &p)
 {
-    using namespace rf;
     if (!d_record || !g || !sp || !sp->d_cam_ori) return SDB_EINVAL;
     if (!g->d_grad_net_out || !g->d_bwd_pack || !g->d_table || !g->d_grad_table || !g->d_grad_global_enc || !g->d_grad_w1ext ||
         !g->d_grad_wh || !g->d_grad_wsig || !g->d_grad_wout || !g->d_grad_sky || !g->d_grad_sky_avg || !g->d_workspace)
         return SDB_EINVAL;
-    cudaStream_t st = (cudaStream_t)stream;
-    Params p;
     {
         const int rc = params_from_abi(sp, p);
         if (rc != SDB_OK) return rc;
@@ -437,137 +459,174 @@ static int render_backward(const sdb_render_params *sp, const void *d_record, co
     if (g->bwd_pack_stride < 0 || (p.n_img > 1 && g->bwd_pack_stride > 0 && g->bwd_pack_stride < packBytes<kBwd>(2))) return SDB_EINVAL;
     for (int k = 0; k < 5; k++)
         if (gstride[k] < 0 || (p.n_img > 1 && gstride[k] < kRenderGradSize[k])) return SDB_EINVAL;
-    uint8_t *rec = (uint8_t *)const_cast<void *>(d_record);
-    const RecordLayout rl = record_layout(p.n_img, p.n_tiles, p.S);
-    bind_record(p, rec, rl);
-    const int32_t *hdr = reinterpret_cast<const int32_t *>(rec + rl.hdr);
-    const long long tpi = p.n_tiles / p.n_img, hw = (long long)p.H * p.W;
-    const BwdLayout bl = bwd_layout(tpi, p.S, sp->L, p.log2_T);
-    uint8_t *ws = (uint8_t *)g->d_workspace;
-    float *dc32 = reinterpret_cast<float *>(ws + bl.dc32);
-    uint16_t *dc16 = reinterpret_cast<uint16_t *>(ws + bl.dc16);
-    float *dsig32 = reinterpret_cast<float *>(ws + bl.dsig32);
-    uint16_t *dsig16 = reinterpret_cast<uint16_t *>(ws + bl.dsig16);
-    uint16_t *dz = reinterpret_cast<uint16_t *>(ws + bl.dz);
-    float *dx0 = reinterpret_cast<float *>(ws + bl.dx0);
-    float *dt3 = reinterpret_cast<float *>(ws + bl.dt3);
-    p.tr.dc = dc32; p.tr.dsig = dsig32; p.tr.dz = dz; p.tr.dx0 = dx0;
-    p.pack = (const uint8_t *)g->d_bwd_pack; p.pack_stride = g->bwd_pack_stride;
+    return SDB_OK;
+}
 
-    const bool timing0 = getenv("SDB_TIMING") != nullptr;
-    cudaEvent_t tev0 = nullptr;
-    if (timing0) { cudaEventCreate(&tev0); cudaEventRecord(tev0, st); }
-    // The live-tile counts of the recorded pass stay ON THE DEVICE (record header): every kernel below is launched over one
-    // view's capacity and reads its image's {first, count} there, so this call never synchronises -- the host can queue the whole
+// lays out the workspace and zeroes every output the views accumulate into
+static int backward_begin(const sdb_render_params *sp, const Params &p, const sdb_render_grads *g, const int64_t *gstride,
+                          BwdBatch &b, cudaStream_t st)
+{
+    b.g = g; b.gstride = gstride;
+    b.tpi = p.n_tiles / p.n_img; b.hw = (long long)p.H * p.W;
+    const BwdLayout bl = bwd_layout(b.tpi, p.S, sp->L, p.log2_T);
+    uint8_t *ws = (uint8_t *)g->d_workspace;
+    b.dc32 = reinterpret_cast<float *>(ws + bl.dc32);
+    b.dc16 = reinterpret_cast<uint16_t *>(ws + bl.dc16);
+    b.dsig32 = reinterpret_cast<float *>(ws + bl.dsig32);
+    b.dsig16 = reinterpret_cast<uint16_t *>(ws + bl.dsig16);
+    b.dz = reinterpret_cast<uint16_t *>(ws + bl.dz);
+    b.dx0 = reinterpret_cast<float *>(ws + bl.dx0);
+    b.dt3 = reinterpret_cast<float *>(ws + bl.dt3);
+    b.timing = getenv("SDB_TIMING") != nullptr;
+    b.tev0 = nullptr;
+    if (b.timing) { cudaEventCreate(&b.tev0); cudaEventRecord(b.tev0, st); }
+    // The live-tile counts of the recorded pass stay ON THE DEVICE (record header): every kernel of a view is launched over one
+    // view's capacity and reads its image's {first, count} there, so a backward never synchronises -- the host can queue the whole
     // backward (and the torch ops behind it) while the forward kernel is still running, which is what makes the step time
     // independent of host speed.
-    const long long cap_items = tpi * p.S;
     const size_t table_bytes = ((size_t)sp->L << p.log2_T) * 8 * 4;
-
     for (int i = 0; i < p.n_img; i++)
         SDB_CUDA(cudaMemsetAsync(g->d_grad_sky_avg + i * gstride[4], 0, (size_t)kOutC * 4, st));
     SDB_CUDA(cudaMemsetAsync(g->d_grad_global_enc, 0, 8, st));
-    SDB_CUDA(cudaMemsetAsync(dt3, 0, table_bytes, st));
+    SDB_CUDA(cudaMemsetAsync(b.dt3, 0, table_bytes, st));
     for (int i = 0; i < p.n_img; i++) {
         SDB_CUDA(cudaMemsetAsync(g->d_grad_w1ext + i * gstride[0], 0, (size_t)kRenderGradSize[0] * 4, st));
         SDB_CUDA(cudaMemsetAsync(g->d_grad_wh + i * gstride[1], 0, (size_t)kRenderGradSize[1] * 4, st));
         SDB_CUDA(cudaMemsetAsync(g->d_grad_wsig + i * gstride[2], 0, (size_t)kRenderGradSize[2] * 4, st));
         SDB_CUDA(cudaMemsetAsync(g->d_grad_wout + i * gstride[3], 0, (size_t)kRenderGradSize[3] * 4, st));
     }
+    b.mark(-1, st);
+    return SDB_OK;
+}
 
-    // SDB_TIMING=1: per-stage device times on stderr, summed over the images (diagnostics; synchronises)
-    const bool timing = getenv("SDB_TIMING") != nullptr;
-    std::vector<cudaEvent_t> tev;
-    auto mark = [&]() { if (timing) { tev.emplace_back(); cudaEventCreate(&tev.back()); cudaEventRecord(tev.back(), st); } };
-    mark();
-    for (int i = 0; i < p.n_img; i++) {
-        const int32_t *view = hdr + 1 + 2 * i;      // {first live-list position, live tiles} of image i
-        // 1. compositing backward over image i's tiles (every tile: sky-only tiles still feed dL/dsky)
-        {
-            Params pi = p;
-            pi.n_img = 1; pi.n_tiles = (int)tpi; pi.view = view;
-            pi.cam_ori = p.cam_ori + 3 * i;
-            pi.sky = p.sky + i * hw * kOutC; pi.sky_avg = p.sky_avg + i * kOutC;
-            pi.tr.tile_work = p.tr.tile_work + i * tpi;
-            composite_backward_kernel<<<(unsigned)tpi, 256, 0, st>>>(pi, g->d_grad_net_out + i * hw * kOutC, g->d_grad_sky + i * hw * kOutC,
-                                                                     g->d_grad_sky_avg + i * gstride[4], dc32, dc16, dsig32, dsig16);
-            SDB_CHECK_LAUNCH();
-        }
-        mark();
-        // 2. data-gradient chain on the tensor-core engine: one work item per (live tile, sample step) of image i -- the slot
-        //    index (work * 1 + 0) * 128 + row of such an item IS the workspace's (tile * S + step) * 128 + row
-        Params pv = p;
-        pv.view = view;
-        pv.n_live = view + 1;
-        {
-            Params pc = pv;
-            pc.work_mult = p.S;
-            pc.S = 1;
-            pc.tr.slot_cap = cap_items * kRows;      // layer stride of dZ in the (one-view) workspace
-            const int grid = cap_items < sdb_num_sms() ? (int)cap_items : sdb_num_sms();      // items beyond count * S do not exist: CTAs find none
-            const int rc = launch_bwd_chain(pc, grid, st);
-            if (rc != SDB_OK) return rc;
-        }
-        mark();
-        // 3a. scatter image i's feature gradients into the pre-blended table gradient (shared by all images)
-        {
-            dim3 grid((unsigned)((cap_items * kRows + 255) / 256), kLevels);
-            // SDB_TABLE_AGG_LEVELS: tuning knob (levels 0..n-1 use the warp-aggregated scatter); the default was chosen on the
-            // previous GPU generation and is carried over, not re-measured on H100
-            int agg_levels = 12;
-            if (const char *e = getenv("SDB_TABLE_AGG_LEVELS")) agg_levels = atoi(e);
-            table3_backward_kernel<<<grid, 256, 0, st>>>(pv, dx0, dt3, agg_levels);
-            SDB_CHECK_LAUNCH();
-        }
-        mark();
-        // 4. image i's weight gradients on the tensor cores (its live items, nothing else: no padding rows to zero).
-        //    A = the record (the image's items start at view[0] * S), Z = the workspace.
-        {
-            const long long cap = p.tr.slot_cap, wcap = cap_items * kRows;
-            float *w1ext = g->d_grad_w1ext + i * gstride[0], *wh = g->d_grad_wh + i * gstride[1];
-            float *wsig = g->d_grad_wsig + i * gstride[2], *wout = g->d_grad_wout + i * gstride[3];
-            WgJob jobs[kWgMaxJobs];
-            int nj = 0;
-            add_jobs(jobs, nj, p.tr.x0, kX0Cols, dz, kHidden, w1ext, kHidden);                                             // fc_1 | fc_m_a | bias
-            for (int k = 0; k < 5; k++)                                                                                    // fc_2 .. fc_6
-                add_jobs(jobs, nj, p.tr.act + (size_t)k * cap * kActCols, kActCols, dz + (size_t)(k + 1) * wcap * kHidden, kHidden,
-                         wh + (size_t)k * kHidden * kActCols, kHidden);
-            add_jobs(jobs, nj, p.tr.act + (size_t)5 * cap * kActCols, kActCols, dc16, kOutC, wout, kOutC);                // fc_out_c
-            add_jobs(jobs, nj, p.tr.act + (size_t)3 * cap * kActCols, kActCols, dsig16, 8, wsig, 8);                      // fc_sigma
-            const int rc = launch_wgrad(jobs, nj, view, p.S, cap_items, st);
-            if (rc != SDB_OK) return rc;
-        }
-        mark();
-    }
-    // 3b. table gradient of the batch: transpose of the pre-blend, scene code (once for all images)
+// stages 1-4 of batch view i over image r of the record p is bound to (p: that record's images, with the backward pack of
+// image r at p.pack + r * p.pack_stride and the workspace in p.tr)
+static int backward_view(const Params &p, int r, int i, BwdBatch &b, cudaStream_t st)
+{
+    const sdb_render_grads *g = b.g;
+    const int64_t *gstride = b.gstride;
+    const long long tpi = b.tpi, hw = b.hw;
+    const long long cap_items = tpi * p.S;
+    const int32_t *view = p.n_live + 1 + 2 * r;      // {first live-list position, live tiles} of image r (record header)
+    // 1. compositing backward over image r's tiles (every tile: sky-only tiles still feed dL/dsky)
     {
-        int rc = sdb_preblend_table(dt3, g->d_grad_table, sp->L, p.log2_T, p.level_S, p.base_res, p.genc, stream);
+        Params pi = p;
+        pi.n_img = 1; pi.n_tiles = (int)tpi; pi.view = view;
+        pi.cam_ori = p.cam_ori + 3 * r;
+        pi.sky = p.sky + r * hw * kOutC; pi.sky_avg = p.sky_avg + r * kOutC;
+        pi.tr.tile_work = p.tr.tile_work + r * tpi;
+        composite_backward_kernel<<<(unsigned)tpi, 256, 0, st>>>(pi, g->d_grad_net_out + i * hw * kOutC, g->d_grad_sky + i * hw * kOutC,
+                                                                 g->d_grad_sky_avg + i * b.gstride[4], b.dc32, b.dc16, b.dsig32, b.dsig16);
+        SDB_CHECK_LAUNCH();
+    }
+    b.mark(0, st);
+    // 2. data-gradient chain on the tensor-core engine: one work item per (live tile, sample step) of image r -- the slot
+    //    index (work * 1 + 0) * 128 + row of such an item IS the workspace's (tile * S + step) * 128 + row
+    Params pv = p;
+    pv.view = view;
+    pv.n_live = view + 1;
+    {
+        Params pc = pv;
+        pc.work_mult = p.S;
+        pc.S = 1;
+        pc.tr.slot_cap = cap_items * kRows;      // layer stride of dZ in the (one-view) workspace
+        const int grid = cap_items < sdb_num_sms() ? (int)cap_items : sdb_num_sms();      // items beyond count * S do not exist: CTAs find none
+        const int rc = launch_bwd_chain(pc, grid, st);
+        if (rc != SDB_OK) return rc;
+    }
+    b.mark(1, st);
+    // 3a. scatter image r's feature gradients into the pre-blended table gradient (shared by all views)
+    {
+        dim3 grid((unsigned)((cap_items * kRows + 255) / 256), kLevels);
+        // SDB_TABLE_AGG_LEVELS: tuning knob (levels 0..n-1 use the warp-aggregated scatter); the default was chosen on the
+        // previous GPU generation and is carried over, not re-measured on H100
+        int agg_levels = 12;
+        if (const char *e = getenv("SDB_TABLE_AGG_LEVELS")) agg_levels = atoi(e);
+        table3_backward_kernel<<<grid, 256, 0, st>>>(pv, b.dx0, b.dt3, agg_levels);
+        SDB_CHECK_LAUNCH();
+    }
+    b.mark(2, st);
+    // 4. view i's weight gradients on the tensor cores (its live items, nothing else: no padding rows to zero).
+    //    A = the record (the image's items start at view[0] * S), Z = the workspace.
+    {
+        const long long cap = p.tr.slot_cap, wcap = cap_items * kRows;
+        float *w1ext = g->d_grad_w1ext + i * gstride[0], *wh = g->d_grad_wh + i * gstride[1];
+        float *wsig = g->d_grad_wsig + i * gstride[2], *wout = g->d_grad_wout + i * gstride[3];
+        WgJob jobs[kWgMaxJobs];
+        int nj = 0;
+        add_jobs(jobs, nj, p.tr.x0, kX0Cols, b.dz, kHidden, w1ext, kHidden);                                           // fc_1 | fc_m_a | bias
+        for (int k = 0; k < 5; k++)                                                                                    // fc_2 .. fc_6
+            add_jobs(jobs, nj, p.tr.act + (size_t)k * cap * kActCols, kActCols, b.dz + (size_t)(k + 1) * wcap * kHidden, kHidden,
+                     wh + (size_t)k * kHidden * kActCols, kHidden);
+        add_jobs(jobs, nj, p.tr.act + (size_t)5 * cap * kActCols, kActCols, b.dc16, kOutC, wout, kOutC);              // fc_out_c
+        add_jobs(jobs, nj, p.tr.act + (size_t)3 * cap * kActCols, kActCols, b.dsig16, 8, wsig, 8);                    // fc_sigma
+        const int rc = launch_wgrad(jobs, nj, view, p.S, cap_items, st);
+        if (rc != SDB_OK) return rc;
+    }
+    b.mark(3, st);
+    return SDB_OK;
+}
+
+// 3b. table gradient of the batch: transpose of the pre-blend, scene code (once for all views); n_live = the header of the
+// record last differentiated (reported with SDB_TIMING)
+static int backward_finish(const sdb_render_params *sp, const Params &p, BwdBatch &b, const int32_t *n_live, cudaStream_t st)
+{
+    const sdb_render_grads *g = b.g;
+    {
+        int rc = sdb_preblend_table(b.dt3, g->d_grad_table, sp->L, p.log2_T, p.level_S, p.base_res, p.genc, st);
         if (rc != SDB_OK) return rc;
         const size_t n = (size_t)sp->L << p.log2_T;
-        genc_backward_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(g->d_table, dt3, sp->L, p.log2_T, p.level_S, p.base_res,
+        genc_backward_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(g->d_table, b.dt3, sp->L, p.log2_T, p.level_S, p.base_res,
                                                                           p.genc, g->d_grad_global_enc);
         SDB_CHECK_LAUNCH();
     }
-    mark();
-    if (timing) {
+    b.mark(4, st);
+    if (b.timing) {
         cudaStreamSynchronize(st);
-        float ms[4] = {0, 0, 0, 0}, untable = 0.0f;
-        for (int i = 0; i < p.n_img; i++)
-            for (int k = 0; k < 4; k++) {
-                float t = 0.0f;
-                cudaEventElapsedTime(&t, tev[4 * i + k], tev[4 * i + k + 1]);
-                ms[k] += t;
-            }
-        cudaEventElapsedTime(&untable, tev[4 * p.n_img], tev[4 * p.n_img + 1]);
-        float pre = 0.0f;
-        if (tev0) { cudaEventElapsedTime(&pre, tev0, tev[0]); cudaEventDestroy(tev0); }
-        int32_t n_live = 0;
-        cudaMemcpy(&n_live, rec + rl.hdr, 4, cudaMemcpyDeviceToHost);
-        fprintf(stderr, "[sdb timing] backward: prologue %.3f ms, compositing %.3f ms, chain %.3f ms, table %.3f ms, weight GEMMs %.3f ms (n_live %d)\n",
-                pre, ms[0], ms[1], ms[2] + untable, ms[3], n_live);
-        for (cudaEvent_t e : tev) cudaEventDestroy(e);
+        float ms[6] = {0, 0, 0, 0, 0, 0}, pre = 0.0f;
+        for (size_t j = 1; j < b.tev.size(); j++) {
+            float t = 0.0f;
+            cudaEventElapsedTime(&t, b.tev[j - 1].second, b.tev[j].second);
+            ms[b.tev[j].first] += t;
+        }
+        if (b.tev0) { cudaEventElapsedTime(&pre, b.tev0, b.tev[0].second); cudaEventDestroy(b.tev0); }
+        int32_t live = 0;
+        cudaMemcpy(&live, n_live, 4, cudaMemcpyDeviceToHost);
+        fprintf(stderr, "[sdb timing] backward: prologue %.3f ms, compositing %.3f ms, chain %.3f ms, table %.3f ms, weight GEMMs %.3f ms (n_live %d)",
+                pre, ms[0], ms[1], ms[2] + ms[4], ms[3], live);
+        if (ms[5] > 0.0f) fprintf(stderr, ", recompute forward %.3f ms", ms[5]);
+        fprintf(stderr, "\n");
+        for (auto &e : b.tev) cudaEventDestroy(e.second);
     }
     return SDB_OK;
+}
+}  // namespace rf
+
+static int render_backward(const sdb_render_params *sp, const void *d_record, const sdb_render_grads *g, const int64_t *gstride,
+                           void *stream)
+{
+    using namespace rf;
+    Params p;
+    {
+        const int rc = backward_check(sp, d_record, g, gstride, p);
+        if (rc != SDB_OK) return rc;
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    uint8_t *rec = (uint8_t *)const_cast<void *>(d_record);
+    const RecordLayout rl = record_layout(p.n_img, p.n_tiles, p.S);
+    bind_record(p, rec, rl);
+    BwdBatch b;
+    {
+        const int rc = backward_begin(sp, p, g, gstride, b, st);
+        if (rc != SDB_OK) return rc;
+    }
+    p.tr.dc = b.dc32; p.tr.dsig = b.dsig32; p.tr.dz = b.dz; p.tr.dx0 = b.dx0;
+    p.pack = (const uint8_t *)g->d_bwd_pack; p.pack_stride = g->bwd_pack_stride;
+    for (int i = 0; i < p.n_img; i++) {
+        const int rc = backward_view(p, i, i, b, st);
+        if (rc != SDB_OK) return rc;
+    }
+    return backward_finish(sp, p, b, p.n_live, st);
 }
 
 extern "C" int sdb_render_rays_backward(const sdb_render_params *sp, const void *d_record, const sdb_render_grads *g, void *stream)
@@ -582,6 +641,63 @@ extern "C" int sdb_render_rays_backward_views(const sdb_render_params *sp, const
     if (!vg) return SDB_EINVAL;
     const int64_t stride[5] = {vg->w1ext_stride, vg->wh_stride, vg->wsig_stride, vg->wout_stride, vg->sky_avg_stride};
     return render_backward(sp, d_record, &vg->g, stride, stream);
+}
+
+// The backward of a forward that kept no record: view by view, the recording forward rebuilds the view's record in
+// d_view_record (one view's size), then that view's stages run over it.  The forward's outputs it recomputes (net_out; depth,
+// weights and the like are not asked for) go to the compositing gradient's part of the workspace, which is free until the
+// view's stage 1 -- the caller's outputs are left as they are.
+extern "C" int sdb_render_rays_backward_recompute(const sdb_render_params *sp, void *d_view_record, const sdb_render_view_grads *vg,
+                                                  void *stream)
+{
+    using namespace rf;
+    if (!vg) return SDB_EINVAL;
+    const int64_t stride[5] = {vg->w1ext_stride, vg->wh_stride, vg->wsig_stride, vg->wout_stride, vg->sky_avg_stride};
+    const sdb_render_grads *g = &vg->g;
+    Params p;
+    {
+        const int rc = backward_check(sp, d_view_record, g, stride, p);
+        if (rc != SDB_OK) return rc;
+    }
+    // the forward's rules (sdb_render_rays_train_forward)
+    if (sp->precision == 1) return SDB_EUNSUPPORTED;
+    const int parts = sp->precision == 0 ? 1 : 2;
+    if (p.n_img > 1 && (p.pack_stride < 0 || (p.pack_stride > 0 && p.pack_stride < packBytes<kRender>(parts)))) return SDB_EINVAL;
+    cudaStream_t st = (cudaStream_t)stream;
+    BwdBatch b;
+    {
+        const int rc = backward_begin(sp, p, g, stride, b, st);
+        if (rc != SDB_OK) return rc;
+    }
+    uint8_t *rec = (uint8_t *)d_view_record;
+    const long long tpi = b.tpi, hw = b.hw;
+    const RecordLayout rl = record_layout(1, tpi, p.S);
+    for (int i = 0; i < p.n_img; i++) {
+        // view i of the batch as a one-image pass: its rays, uniforms, camera, sky and pack
+        Params pi = p;
+        pi.n_img = 1; pi.n_tiles = (int)tpi;
+        pi.voxel_id = p.voxel_id + i * hw * p.M;
+        pi.depth2 = p.depth2 + i * 2 * hw * p.M;
+        pi.raydirs = p.raydirs + i * hw * 3;
+        if (p.uniforms) pi.uniforms = p.uniforms + i * hw * (p.S + 1);
+        pi.cam_ori = p.cam_ori + 3 * i;
+        pi.sky = p.sky + i * hw * kOutC; pi.sky_avg = p.sky_avg + i * kOutC;
+        pi.pack = p.pack + i * p.pack_stride; pi.pack_stride = 0;
+        pi.net_out = b.dc32;      // tiles * S * 128 * 64 floats >= H * W * 64: every ray's output fits
+        pi.depth_out = pi.total_weight = pi.weights_out = pi.rdepth_out = nullptr;
+        bind_record(pi, rec, rl);
+        {
+            int rc = launch_train_prepass(pi, reinterpret_cast<int32_t *>(rec + rl.hdr), reinterpret_cast<int32_t *>(rec + rl.tile_list), st);
+            if (rc == SDB_OK) rc = launch_train_forward(pi, sp->precision, tpi < sdb_num_sms() ? (int)tpi : sdb_num_sms(), st);
+            if (rc != SDB_OK) return rc;
+        }
+        b.mark(5, st);
+        pi.tr.dc = b.dc32; pi.tr.dsig = b.dsig32; pi.tr.dz = b.dz; pi.tr.dx0 = b.dx0;
+        pi.pack = (const uint8_t *)g->d_bwd_pack + i * g->bwd_pack_stride; pi.pack_stride = 0;
+        const int rc = backward_view(pi, 0, i, b, st);
+        if (rc != SDB_OK) return rc;
+    }
+    return backward_finish(sp, p, b, reinterpret_cast<const int32_t *>(rec + rl.hdr), st);
 }
 
 // ---- sky branch (a9) backward: SKYMLP data-gradient chain on the tensor-core engine + weight-gradient GEMMs -------------

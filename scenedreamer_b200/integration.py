@@ -54,6 +54,13 @@ def train_views_enabled():
     return os.environ.get('SDB200_TRAIN_VIEWS', '0') not in ('0', 'false', 'False', 'off', '')
 
 
+def train_recompute_enabled():
+    """SDB200_TRAIN_RECOMPUTE=1: the training passes keep no per-sample record from forward to backward; the backward
+    rebuilds one view's record at a time (render.render_rays_train(recompute=True)), so a batch of views needs one view's
+    record instead of one per view, for one more recording forward per view.  Off by default."""
+    return os.environ.get('SDB200_TRAIN_RECOMPUTE', '0') not in ('0', 'false', 'False', 'off', '')
+
+
 # ------------------------------------------------------------------------------------------------
 # per-instance state
 # ------------------------------------------------------------------------------------------------
@@ -87,7 +94,7 @@ class _FusedState:
         self.frame = _FrameCache()
         self.stats = {'fused_calls': 0, 'frame_launches': 0, 'tile_hits': 0, 'train_calls': 0, 'reference_calls': 0,
                       'cnn_frame_launches': 0, 'cnn_tile_hits': 0, 'cnn_calls': 0, 'cnn_reference_calls': 0,
-                      'cnn_train_calls': 0}
+                      'cnn_train_calls': 0, 'train_recompute_calls': 0}
 
     @property
     def lut(self):
@@ -296,7 +303,9 @@ def fused_forward_perpix(self, blk_feats, voxel_id, depth2, raydirs, cam_ori_t, 
         sky_attr = getattr(self, 'sky_avg', None)
         sky_avg = None if sky_attr is None else sky_attr.reshape(-1, 64).expand(N, 64)
         args = ([float(v) for v in self.voxel.voxel_t.shape], st.lut, he.per_level_scale)
-        kw.update(base_res=he.base_resolution, log2_T=he.log2_hashmap_size, L=he.num_levels, precision=prec)
+        recompute = train_recompute_enabled()
+        st.stats['train_recompute_calls'] += int(recompute)
+        kw.update(base_res=he.base_resolution, log2_T=he.log2_hashmap_size, L=he.num_levels, precision=prec, recompute=recompute)
         if train_views:
             out = render.render_rays_train(P, voxel_id.contiguous(), depth2.contiguous(), raydirs.contiguous(), cam_ori_t, z,
                                            global_enc[:1], *args, uniforms=uniforms, sky_avg=sky_avg, **kw)

@@ -508,18 +508,29 @@ class _FusedRenderTrainFn(torch.autograd.Function):
             wts = torch.empty(N, H, W, S, 1, dtype=torch.float32, device=dev)
             rdp = torch.empty(N, H, W, S, 1, dtype=torch.float32, device=dev)
             ws = torch.empty(int(L.sdb_render_workspace_bytes(N, H, W)), dtype=torch.uint8, device=dev)
-            record = _take_scratch(L.sdb_render_train_record_bytes(N, H, W, S), dev, 'record')
+            recompute = bool(cfg.get('recompute'))
+            # recompute: no record now -- the backward rebuilds each view's record just before differentiating it, from what
+            # ctx.keep holds alive (rays, uniforms, camera origins, packs, table3, sky, sky_avg).  The inference kernel without
+            # early termination computes what the recording kernel computes, bit for bit.
+            record = None if recompute else _take_scratch(L.sdb_render_train_record_bytes(N, H, W, S), dev, 'record')
             prm, keep = _RenderParams(), []
             _fill_render_params(prm, keep, voxel_id, depth2, raydirs, cam_ori, genc_, cfg['voxel_dims'], lut, pack, sky_, sky_avg_,
                                 table3=table3, S=S, sample_depth=cfg['sample_depth'], dists_scale=cfg['dists_scale'],
                                 uniforms=cfg.get('uniforms'), precision=prec, per_level_scale=cfg['per_level_scale'],
                                 base_res=cfg['base_res'], log2_T=cfg['log2_T'], L=cfg['L'], net_out=net_out, depth=depth, tw=tw,
                                 wts=wts, rdp=rdp, ws=ws)
-            _lib.check(L.sdb_render_rays_train_forward(ctypes.byref(prm), _ptr(record), _stream(dev)),
-                       'sdb_render_rays_train_forward')
+            if recompute:
+                _lib.check(L.sdb_render_rays_forward(ctypes.byref(prm), _stream(dev)), 'sdb_render_rays_forward')
+            else:
+                _lib.check(L.sdb_render_rays_train_forward(ctypes.byref(prm), _ptr(record), _stream(dev)),
+                           'sdb_render_rays_train_forward')
         ctx.cfg, ctx.prm, ctx.keep = cfg, prm, keep + [cam_ori, lut, pack, table3, net_out, depth, tw, wts, rdp, ws, genc_, sky_,
                                                        sky_avg_]
-        ctx.record = record
+        ctx.record, ctx.recompute, ctx.released = record, recompute, False
+        if recompute:
+            # the backward reads the caller's rays, uniforms, camera origins and sky features again: saved so that autograd
+            # refuses a backward after one of them was modified in place instead of differentiating another pass
+            ctx.save_for_backward(voxel_id, depth2, raydirs, sky_, sky_avg_, *[t for t in keep if t is not None])
         ctx.saved = (embeddings_, w1_, wh_, wsig_, wout_)
         ctx.shapes = (tuple(fc_m_a.shape), tuple(wsig.shape), tuple(bsig.shape), tuple(sky.shape), tuple(sky_avg.shape),
                       tuple(genc.shape), tuple(wh.shape), tuple(bh.shape))
@@ -529,9 +540,11 @@ class _FusedRenderTrainFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_net_out, *_unused):
         L = _lib.lib()
-        if ctx.record is None:
+        if ctx.released:
             raise RuntimeError('fused render: the training record of this pass was released by its first backward '
                                '(retain_graph / double backward are not supported on the fused path)')
+        if ctx.recompute:
+            ctx.saved_tensors      # the version check of the inputs the recompute reads (RuntimeError if one was modified)
         cfg, prm = ctx.cfg, ctx.prm
         embeddings_, w1_, wh_, wsig_, wout_ = ctx.saved
         dev = embeddings_.device
@@ -560,12 +573,19 @@ class _FusedRenderTrainFn(torch.autograd.Function):
             gr.d_grad_sky, gr.d_grad_sky_avg, gr.d_workspace = _ptr(g_sky), _ptr(g_sky_avg), _ptr(wsb)
             vg.w1ext_stride, vg.wh_stride, vg.wsig_stride = g_w1ext.stride(0), g_wh.stride(0), g_wsig.stride(0)
             vg.wout_stride, vg.sky_avg_stride = g_wout.stride(0), g_sky_avg.stride(0)
-            _lib.check(L.sdb_render_rays_backward_views(ctypes.byref(prm), _ptr(ctx.record), ctypes.byref(vg), _stream(dev)),
-                       'sdb_render_rays_backward_views')
+            if ctx.recompute:
+                # one view's record, rebuilt for every view in turn
+                record = _take_scratch(L.sdb_render_train_record_bytes(1, H, W, S), dev, 'record')
+                _lib.check(L.sdb_render_rays_backward_recompute(ctypes.byref(prm), _ptr(record), ctypes.byref(vg), _stream(dev)),
+                           'sdb_render_rays_backward_recompute')
+            else:
+                record = ctx.record
+                _lib.check(L.sdb_render_rays_backward_views(ctypes.byref(prm), _ptr(record), ctypes.byref(vg), _stream(dev)),
+                           'sdb_render_rays_backward_views')
         # stream-ordered reuse: the next forward / backward run on the same stream after these kernels
         _give_scratch(wsb, 'bwd')
-        _give_scratch(ctx.record, 'record')
-        ctx.record = None
+        _give_scratch(record, 'record')
+        ctx.record, ctx.released = None, True
         s_fcma, s_wsig, s_bsig, s_sky, s_skyavg, s_genc, s_wh, s_bh = ctx.shapes
         n_lab = s_fcma[1]
         d_genc = torch.zeros(s_genc, dtype=torch.float32, device=dev)
@@ -648,7 +668,8 @@ def sky_features_train(P, raydirs, z, prefix='sky_net'):
 
 def render_rays_train(P, voxel_id, depth2, raydirs, cam_ori, z, global_enc, voxel_dims, label_lut, per_level_scale,
                       num_samples=24, sample_depth=3.0, dists_scale=0.25, uniforms=None, base_res=16, log2_T=19, L=16,
-                      prefix='render_net', sky_prefix='sky_net', sky_impl='native', sky_avg=None, precision=PRECISION_FP16X3):
+                      prefix='render_net', sky_prefix='sky_net', sky_impl='native', sky_avg=None, precision=PRECISION_FP16X3,
+                      recompute=False):
     """Differentiable fused a2-a12 for N views of ONE scene in one recorded pass (voxel_id [N,H,W,M,1], z [N,256],
     global_enc [1,2] or N equal rows): gradients reach P['hash_encoder.embeddings'], P['render_net.*'], P['sky_net.*'], z
     and global_enc (everything Generator._forward_perpix differentiates under train.py), summed over the views as autograd
@@ -659,15 +680,23 @@ def render_rays_train(P, voxel_id, depth2, raydirs, cam_ori, z, global_enc, voxe
     precision: of the recording forward's MLP, PRECISION_FP16X3 (fp32-grade) or PRECISION_FP16 (one fp16 pass, for
     mixed-precision training); the sky branch and the backward are fp32-grade either way.  The torch glue runs in fp32 with
     autocast off, whatever the caller's autocast state and the dtypes of z / global_enc / sky_avg; autograd hands their
-    gradients back in their own dtypes."""
+    gradients back in their own dtypes.
+    recompute: False = the forward keeps a per-sample record of every view until the backward (about 3.9 KB per sample:
+    6.9 GB per 262x262 view at 24 spp); True = it keeps none, and the backward rebuilds one view's record at a time just
+    before differentiating that view (sdb_render_rays_backward_recompute), so the record no longer grows with the batch.
+    The outputs are the same bit for bit and the gradients differ only in the order of fp32 atomics; the cost is one more
+    recording forward per view.  The backward reads voxel_id, depth2, raydirs, uniforms, cam_ori and the sky features again:
+    modifying one of them in place between forward and backward makes the backward raise, as for any tensor autograd saved.
+    In either mode a second backward through the same graph (retain_graph) raises."""
     with torch.autocast('cuda', enabled=False):
         return _render_rays_train(P, voxel_id, depth2, raydirs, cam_ori, z.float(), global_enc.float(), voxel_dims, label_lut,
                                   per_level_scale, num_samples, sample_depth, dists_scale, uniforms, base_res, log2_T, L, prefix,
-                                  sky_prefix, sky_impl, None if sky_avg is None else sky_avg.float(), precision)
+                                  sky_prefix, sky_impl, None if sky_avg is None else sky_avg.float(), precision, recompute)
 
 
 def _render_rays_train(P, voxel_id, depth2, raydirs, cam_ori, z, global_enc, voxel_dims, label_lut, per_level_scale, num_samples,
-                       sample_depth, dists_scale, uniforms, base_res, log2_T, L, prefix, sky_prefix, sky_impl, sky_avg, precision):
+                       sample_depth, dists_scale, uniforms, base_res, log2_T, L, prefix, sky_prefix, sky_impl, sky_avg, precision,
+                       recompute):
     p = prefix + '.'
     N = voxel_id.shape[0]
     if z.shape[0] != N:
@@ -684,7 +713,7 @@ def _render_rays_train(P, voxel_id, depth2, raydirs, cam_ori, z, global_enc, vox
         sky_avg = sky_avg.reshape(-1, 64).expand(N, 64)
     cfg = dict(voxel_id=voxel_id, depth2=depth2, raydirs=raydirs, cam_ori=cam_ori, lut=label_lut, voxel_dims=voxel_dims,
                num_samples=num_samples, sample_depth=sample_depth, dists_scale=dists_scale, uniforms=uniforms,
-               per_level_scale=per_level_scale, base_res=base_res, log2_T=log2_T, L=L, precision=precision)
+               per_level_scale=per_level_scale, base_res=base_res, log2_T=log2_T, L=L, precision=precision, recompute=recompute)
     net_out, depth, tw, wts, rdp = _FusedRenderTrainFn.apply(
         cfg, P['hash_encoder.embeddings'], global_enc, P[p + 'fc_1.weight'], P[p + 'fc_1.bias'], P[p + 'fc_m_a.weight'],
         wh, bh, P[p + 'fc_sigma.weight'], P[p + 'fc_sigma.bias'], P[p + 'fc_out_c.weight'], P[p + 'fc_out_c.bias'], sky,
