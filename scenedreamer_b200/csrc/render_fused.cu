@@ -366,6 +366,11 @@ mlp_kernel(const Params p)
     float *sSig = reinterpret_cast<float *>(smem + SM.sig);
     float *sState = reinterpret_cast<float *>(smem + SM.state);
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem + SM.bars);
+    uint32_t *sWalk = reinterpret_cast<uint32_t *>(smem + SM.walk);
+    // the weight ring: 16 KB slots, each holding one stage (k16 slabs of one 64-column block, block_stages / stage_slabs)
+    constexpr uint32_t kSlot = 16384, kSlabB = 2048 * PARTS;       // ring slot; one k16 slab of a 64-column block
+    constexpr int kSps = kSlot / kSlabB;                           // slabs per ring slot
+    constexpr int kStepStages = step_stages<MODE>(kSps);
     // Early termination (north star: "early termination"; inference render only).  stop_step[buf] = number of sample
     // steps the tile in state buffer `buf` executes (S until decided).  The epilogue decides during the compositing of
     // step s ("every live ray has transmittance < early_T") and sets s + 2: by the time ANY role starts step s + 2 it
@@ -415,6 +420,22 @@ mlp_kernel(const Params p)
         for (int i = 0; i < 2; i++) { tc05::mbar_init(&bars[B_STRDY + i], kRows); tc05::mbar_init(&bars[B_STFREE + i], kEpiThreads); }
         tc05::mbar_init(&bars[B_COMP], kEpiThreads);
         tc05::fence_mbar_init();
+        // the ring stages of one sample step, the same for every step and image: per layer and row block, the layer's bytes in
+        // pack order (the pack is stored in streaming order, wpack_off) cut at stage boundaries.  Entry = pack offset / 2 KB |
+        // bytes / 2 KB << 16, so that a refill is one shared load (walking the layers per refill took most of its time).
+        int k = 0;
+        for (int l = 0; l < NL; l++) {
+            const int nK = layerK<MODE>(l) / 16, ncb = layerN<MODE>(l) / 64, nsb = block_stages(nK, kSps);
+            for (int rb = 0; rb < 2; rb++) {
+                uint32_t po = (uint32_t)layerOff<MODE>(l, PARTS);    // the layer again for each row block
+                for (int c = 0; c < ncb; c++)
+                    for (int js = 0; js < nsb; js++) {
+                        const uint32_t bytes = (uint32_t)stage_slabs(nK, kSps, js) * kSlabB;
+                        sWalk[k++] = (po >> 11) | ((bytes >> 11) << 16);
+                        po += bytes;
+                    }
+            }
+        }
     }
     if (tid < 2) { sStop[tid] = RAYQ ? 0x7fffffff : kMaxS + 1; sVote[tid] = 0; sVoted[tid] = 0; }
     if constexpr (RAYQ) {
@@ -800,8 +821,6 @@ mlp_kernel(const Params p)
       // stored while it runs, then block c + 1's group 1 goes to X, and so on.  Every stage is its own commit group, so its
       // ring slot is released (and refilled with a stage of the next block) as soon as its MMAs are done.
       const int t = tid - kMmaWarp0 * 32;
-      constexpr uint32_t kSlot = 16384, kSlabB = 2048 * PARTS;       // ring slot; one k16 slab of a 64-column block
-      constexpr int kSps = kSlot / kSlabB;                           // slabs per ring slot
       static_assert(block_stages(kHidden / 16, kSps) <= 4 && block_stages(kRenderK0 / 16, kSps) <= 4,
                     "the stages of one column block fit the 4-slot ring");
       constexpr bool BIAS = Net<MODE>::NBIAS > 0;
@@ -823,24 +842,14 @@ mlp_kernel(const Params p)
           }
           for (int s = 0; s < SL; s++, n++) {
               if (ESTOP && s >= 2 && s >= sStop[it & 1]) break;
-              // weight loads (thread 0): the stages of a step are, per layer and row block, the layer's bytes in pack order (the
-              // pack is stored in streaming order, wpack_off), cut at stage boundaries.  The next one to load is stage js of a
-              // block of layer pl, row block pr, at byte po of the pack, ring index pq.
-              int pl = 0, pr = 0, js = 0;
-              uint32_t pq = q, po = 0;
+              // weight loads (thread 0): stage pq - q0 of this step's table (sWalk), ring index pq
+              const uint32_t q0 = q;
+              uint32_t pq = q;
               auto produce = [&](uint32_t upto) {
-                  for (; pq < upto && pl < NL; pq++) {
-                      const int nK = layerK<MODE>(pl) / 16;
-                      const uint32_t bytes = (uint32_t)stage_slabs(nK, kSps, js) * kSlabB, slot = pq & 3u;
+                  for (; pq < upto && pq - q0 < (uint32_t)kStepStages; pq++) {
+                      const uint32_t e = sWalk[pq - q0], bytes = (e >> 16) << 11, slot = pq & 3u;
                       tc05::mbar_arrive_expect_tx(&bars[B_WFULL + slot], bytes);
-                      tc05::bulk_g2s(sRing + slot * kSlot, pack + po, bytes, &bars[B_WFULL + slot]);
-                      po += bytes;
-                      if (++js == block_stages(nK, kSps)) js = 0;
-                      if (po == (uint32_t)layerOff<MODE>(pl + 1, PARTS)) {       // end of the layer: again for row block 1, or the next layer
-                          if (pr == 0) po = (uint32_t)layerOff<MODE>(pl, PARTS);
-                          else pl++;
-                          pr ^= 1;
-                      }
+                      tc05::bulk_g2s(sRing + slot * kSlot, pack + ((e & 0xffffu) << 11), bytes, &bars[B_WFULL + slot]);
                   }
               };
               if (t == 0) produce(q + 4);
@@ -902,9 +911,10 @@ mlp_kernel(const Params p)
                           auto release = [&]() {
                               ts.lap(kSplitWait);
                               tc05::named_sync(3, 128);       // every warp is done with the slot
+                              ts.lap(kSplitBarrier);
                               if (t == 0) produce(qr + 5);
                               qr++;
-                              ts.lap(kSplitRetire);
+                              ts.lap(kSplitRefill);
                           };
 #pragma unroll 1
                           for (int k = nsb - 1; k > 0; k--) {
@@ -932,7 +942,7 @@ mlp_kernel(const Params p)
                                   a[i + 1] = __fadd_rn(a[i + 1], bb.y);
                               }
                           }
-                          ts.lap(kSplitRetire);
+                          ts.lap(kSplitReduce);
                           if (c + 1 < ncb) issue(b, 0, ns0);
 #ifndef SDB_AB_NO_ACC
 #pragma unroll
@@ -940,7 +950,7 @@ mlp_kernel(const Params p)
                               *reinterpret_cast<float2 *>(p.acc + (dst + (uint32_t)(tc05::frag_row(ft, i) * kHidden + c * 64 + tc05::frag_col(ft, i)))) =
                                   make_float2(a[i], a[i + 1]);
 #endif
-                          ts.lap(kSplitRetire);
+                          ts.lap(kSplitStore);
                       };
                       issue(x, 0, ns0);
 #pragma unroll 1
@@ -950,7 +960,7 @@ mlp_kernel(const Params p)
                       }
                       __threadfence_block();
                       tc05::named_sync(3, 128);
-                      ts.lap(kSplitRetire);
+                      ts.lap(kSplitBarrier);
                       if (t == 0) SDB_STAMP(n, l, 2 * rb + 1);
                       if (t == 0) SDB_STAMP_SPLIT(n, l, rb, ts);
                       if (t == 0) {

@@ -99,6 +99,24 @@ __host__ __device__ constexpr int stage_slabs(int nK, int sps, int js) {
     return left < sps ? left : sps;
 }
 
+// ring stages of one sample step of network MODE: per layer and row block, the stages of the layer's 64-column blocks
+template <int MODE> __host__ __device__ constexpr int step_stages(int sps) {
+    int n = 0;
+    for (int l = 0; l < Net<MODE>::NL; l++) n += 2 * (layerN<MODE>(l) / 64) * block_stages(layerK<MODE>(l) / 16, sps);
+    return n;
+}
+constexpr int kMaxStepStages = 192;   // the render network at x3 (4 slabs per stage)
+static_assert(step_stages<kRender>(4) <= kMaxStepStages && step_stages<kSky>(4) <= kMaxStepStages &&
+              step_stages<kBwd>(4) <= kMaxStepStages && step_stages<kSkyBwd>(4) <= kMaxStepStages &&
+              step_stages<kRender>(8) <= kMaxStepStages && step_stages<kSky>(8) <= kMaxStepStages,
+              "stage table of one sample step");
+// a layer is whole [64 x 16] blocks of 16-bit parts, so every stage starts and ends on a 2 KB boundary of the pack, and an entry
+// of the table holds the stage's offset and size in 2 KB units in 16 bits each
+static_assert(64 * 16 * 2 == 2048, "stage table entries count 2 KB units");
+static_assert((layerOff<kRender>(Net<kRender>::NL, 2) >> 11) < 65536 && (layerOff<kBwd>(Net<kBwd>::NL, 2) >> 11) < 65536 &&
+              (layerOff<kSky>(Net<kSky>::NL, 2) >> 11) < 65536 && (layerOff<kSkyBwd>(Net<kSkyBwd>::NL, 2) >> 11) < 65536,
+              "stage table offsets fit 16 bits");
+
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}\n" : "=r"(pred));
@@ -107,7 +125,7 @@ __device__ __forceinline__ bool elect_one() {
 
 // ---- shared memory map ---------------------------------------------------------------------------
 struct Smem {
-    uint32_t h_hi, h_lo, ring, fsec, bias, scales, frac, sig, state, bars, stop, sched, total;
+    uint32_t h_hi, h_lo, ring, fsec, bias, scales, frac, sig, state, bars, stop, sched, walk, total;
 };
 __host__ __device__ constexpr Smem smem_map(bool x3) {
     Smem m{};
@@ -124,6 +142,7 @@ __host__ __device__ constexpr Smem smem_map(bool x3) {
     m.bars = o; o += 40 * 8;
     m.stop = o; o += 32;                         // early termination: int stop_step[2] (per tile buffer), int vote[2], int voted[2]
     m.sched = o; o += 32;                        // dynamic tile scheduler: int work[4] (ring), int published
+    m.walk = o; o += kMaxStepStages * 4;         // the weight stages of one sample step (read by the MMA warpgroup's thread 0)
     m.total = o;
     return m;
 }
@@ -247,10 +266,12 @@ __device__ __forceinline__ void acc_ld(const float *src, float (&v)[NV]) {
 //   slot 4 + 2 rb  epilogue of row block rb: accumulators seen        slot 5 + 2 rb: the next layer's operand rows handed over
 //   layer row 7 = the gather role preparing step n: 0 compositing of step n-2 seen, 1 slots refilled, 2 features gathered, 3 operand buffer free
 // and the MMA warpgroup's row-block time (slot 2 rb -> slot 2 rb + 1) split into cycles spent in kSplit* (thread 0's clock):
-//   debug[kSplitBase + ((n - first) * 8 + layer) * 8 + rb * 4 + k]
+//   debug[kSplitBase + (((n - first) * 8 + layer) * 2 + rb) * 8 + k]
+// full-barrier waits, wgmma issue, wait_group, then what follows wait_group: synchronisation inside the warpgroup (ring-slot
+// release and row-block hand-over), weight refills, the block's sums and bias adds, its accumulator-buffer stores
 constexpr int32_t kTraceMagic = 0x7131;
 constexpr int kTraceSteps = 6, kSplitBase = 512;
-enum { kSplitFull = 0, kSplitIssue, kSplitWait, kSplitRetire };   // full-barrier waits, wgmma issue, wait_group, retire / add / store
+enum { kSplitFull = 0, kSplitIssue, kSplitWait, kSplitBarrier, kSplitRefill, kSplitReduce, kSplitStore, kSplitN };
 #ifndef SDB_TIMELINE
 #define SDB_STAMP(n_, layer, slot) do { } while (0)      // compiled out: the stamps cost the epilogue role registers (spills)
 struct TSplit {
@@ -260,8 +281,11 @@ struct TSplit {
 #define SDB_STAMP_SPLIT(n_, layer, rb, ts) do { } while (0)
 #else
 struct TSplit {                                   // cycles since the last lap, charged to category k
-    uint32_t acc[4], t;
-    __device__ __forceinline__ void start() { acc[0] = acc[1] = acc[2] = acc[3] = 0; t = (uint32_t)clock(); }
+    uint32_t acc[kSplitN], t;
+    __device__ __forceinline__ void start() {
+        for (int k = 0; k < kSplitN; k++) acc[k] = 0;
+        t = (uint32_t)clock();
+    }
     __device__ __forceinline__ void lap(int k) { const uint32_t c = (uint32_t)clock(); acc[k] += c - t; t = c; }
 };
 #define SDB_STAMP_SPLIT(n_, layer, rb, ts)                                                                         \
@@ -269,7 +293,7 @@ struct TSplit {                                   // cycles since the last lap, 
         if (p.debug != nullptr && blockIdx.x == 0 && p.debug[60] == kTraceMagic) {                                 \
             const int rel__ = (int)(n_) - p.debug[61];                                                             \
             if (rel__ >= 0 && rel__ < kTraceSteps)                                                                 \
-                for (int k__ = 0; k__ < 4; k__++) p.debug[kSplitBase + (rel__ * 8 + (layer)) * 8 + (rb) * 4 + k__] = (int32_t)(ts).acc[k__]; \
+                for (int k__ = 0; k__ < kSplitN; k__++) p.debug[kSplitBase + ((rel__ * 8 + (layer)) * 2 + (rb)) * 8 + k__] = (int32_t)(ts).acc[k__]; \
         }                                                                                                          \
     } while (0)
 #define SDB_STAMP(n_, layer, slot)                                                                                 \

@@ -29,7 +29,7 @@ fr.frame(cam)
 torch.cuda.synchronize()
 L.sdb_debug_set_progress_buffer(ctypes.c_void_p(0))
 t = buf[64:64 + 6 * 8 * 8].cpu().numpy().astype(np.int64).reshape(6, 8, 8) & 0xffffffff
-sp = buf[512:512 + 6 * 8 * 8].cpu().numpy().astype(np.int64).reshape(6, 8, 2, 4)   # rf_common.cuh kSplitBase
+sp = buf[512:512 + 6 * 8 * 16].cpu().numpy().astype(np.int64).reshape(6, 8, 2, 8)[..., :7]   # rf_common.cuh kSplitBase, kSplit*
 NL = 7
 names = ['fc_1', 'fc_2', 'fc_3', 'fc_4', 'fc_5', 'fc_6', 'out_c']
 
@@ -62,9 +62,13 @@ for s in range(1, 5):
                                                                               [d(t[s, l][0], base) for l in range(NL)]))
 print('step period (MMA warpgroup, fc_1 to fc_1): %s cycles' % [d(t[s + 1, 0][0], t[s, 0][0]) for s in range(0, 5)])
 print('# MMA warpgroup, where a row block\'s time goes (thread 0, cycles, steps %d..%d averaged): full = full-barrier waits,' % (first + 1, first + 4))
-print('#   issue = wgmma issue + commit, wait = wgmma.wait_group, retire = slot release, sums, bias, stores, hand-over')
-print('%-6s %7s %7s %7s %7s %7s | %7s %7s %7s %7s %7s' % ('layer', 'full0', 'issue0', 'wait0', 'retire0', 'sum0', 'full1', 'issue1', 'wait1', 'retire1', 'sum1'))
+print('#   issue = wgmma issue + commit, wait = wgmma.wait_group, then what follows wait_group (retire = the sum of the four):')
+print('#   barrier = synchronisation inside the warpgroup (ring-slot release, row-block hand-over), refill = weight-stage refills,')
+print('#   reduce = the block\'s two-group sum and bias adds, store = accumulator-buffer stores')
+cols = ['full', 'issue', 'wait', 'barrier', 'refill', 'reduce', 'store', 'retire', 'sum']
+print('%-6s %2s %s' % ('layer', 'rb', ' '.join('%7s' % c for c in cols)))
 for l in range(NL):
     m = sp[1:5, l].mean(axis=0)
-    print('%-6s %s | %s' % (names[l], ' '.join('%7d' % v for v in list(m[0]) + [m[0].sum()]),
-                            ' '.join('%7d' % v for v in list(m[1]) + [m[1].sum()])))
+    for rb in range(2):
+        v = list(m[rb]) + [m[rb][3:7].sum(), m[rb].sum()]
+        print('%-6s %2d %s' % (names[l], rb, ' '.join('%7d' % x for x in v)))
