@@ -17,9 +17,9 @@
 //     so compositing is a per-thread running sum (no cross-thread reduction, any S);
 //   * warp roles: 8 epilogue warps (accumulator row -> LeakyReLU -> 16-bit operand in smem; sigma tap;
 //     compositing; warps 0-3 own columns 0..127, warps 4-7 columns 128..255 of the same 128 rows),
-//     one MMA warpgroup (wgmma in 64x64 blocks; its thread 0 also streams the weights into a 4-slot ring
-//     with 1-D bulk TMA copies), 8 gather warps (hash-grid fetch for the NEXT sample step while the MLP
-//     of the current one runs; results wait in registers until the operand buffer is free);
+//     one MMA warpgroup (wgmma in 64x64 blocks), 8 gather warps (hash-grid fetch for the NEXT sample step
+//     while the MLP of the current one runs; results wait in registers until the operand buffer is free),
+//     one producer warpgroup (one thread streams the weights into a 4-slot ring with 1-D bulk TMA copies);
 //   * accumulators: a layer's fp32 [128 x 256] result (128 KB) fits neither next to the operand buffers in
 //     shared memory nor in the registers the three roles share, so the MMA warpgroup writes it to a
 //     per-CTA buffer pair in global memory (L2-resident, ping-pong by layer parity) and the epilogue reads
@@ -419,6 +419,7 @@ mlp_kernel(const Params p)
         }
         for (int i = 0; i < 2; i++) { tc05::mbar_init(&bars[B_STRDY + i], kRows); tc05::mbar_init(&bars[B_STFREE + i], kEpiThreads); }
         tc05::mbar_init(&bars[B_COMP], kEpiThreads);
+        for (int i = 0; i < 4; i++) tc05::mbar_init(&bars[B_WEMPTY + i], 4);
         tc05::fence_mbar_init();
         // the ring stages of one sample step, the same for every step and image: per layer and row block, the layer's bytes in
         // pack order (the pack is stored in streaming order, wpack_off) cut at stage boundaries.  Entry = pack offset / 2 KB |
@@ -808,9 +809,9 @@ mlp_kernel(const Params p)
       // blocks (the sum over K in registers) written once to this CTA's fp32 accumulator buffer (g & 1) in global memory, where
       // the epilogue reads its rows.  A row block is handed over as soon as it is written, so the epilogue of one row block runs
       // while the MMAs of the other do.  Weights go through a 4-slot ring of 16 KB stages (4 k16 slabs of one 64-column block
-      // at x3, 8 at x1; a hidden-layer block at x3 fills the whole ring), one bulk copy each (wpack_off); thread 0 keeps the
-      // ring full, the weights are streamed once per row block.  Named barrier 3 is this warpgroup's (1, 4, 5: epilogue,
-      // 2: gather).
+      // at x3, 8 at x1; a hidden-layer block at x3 fills the whole ring), one bulk copy each (wpack_off); the producer
+      // warpgroup keeps the ring full, the weights are streamed once per row block.  Named barrier 3 is this warpgroup's
+      // (1, 4, 5: epilogue, 2: gather).
       //
       // Numerics: slabs 0..7 of a block and slabs 8..nK-1 are two fresh tensor-core sums d0, d1 (numerics groups), and the
       // block is RN(d0 + d1), or d0 when nK <= 8: the tensor core's own accumulation does not round to nearest, and over a
@@ -819,7 +820,8 @@ mlp_kernel(const Params p)
       // tensor core, exactly) with one more round-to-nearest add.  Two 32-register sets X, Y alternate: block c's group 0 is
       // in X, its group 1 goes to Y; once both are done X = RN(RN(X + Y) + b), block c + 1's group 0 is issued into Y and X is
       // stored while it runs, then block c + 1's group 1 goes to X, and so on.  Every stage is its own commit group, so its
-      // ring slot is released (and refilled with a stage of the next block) as soon as its MMAs are done.
+      // ring slot is released (each warp arrives on the slot's empty barrier once its wait_group says the stage's MMAs are
+      // done) and refilled with a stage of the next block by the producer.
       const int t = tid - kMmaWarp0 * 32;
       static_assert(block_stages(kHidden / 16, kSps) <= 4 && block_stages(kRenderK0 / 16, kSps) <= 4,
                     "the stages of one column block fit the 4-slot ring");
@@ -831,10 +833,9 @@ mlp_kernel(const Params p)
           if (work < 0) break;
           const int tile = RAYQ ? 0 : (ONE_STEP ? work : p.tile_list[rec_work(work) / wmult]);
           const int img = tile_coord(p, tile).img;
-          const uint8_t *pack = p.pack + (long long)img * p.pack_stride;
           if (BIAS && loaded_img != img) {
               // bias table of this image's pack -> shared memory (this warpgroup is its only reader)
-              const float *packB = reinterpret_cast<const float *>(pack + biasOff<MODE>(PARTS));
+              const float *packB = reinterpret_cast<const float *>(p.pack + (long long)img * p.pack_stride + biasOff<MODE>(PARTS));
               tc05::named_sync(3, 128);
               for (int i = t; i < Net<MODE>::NBIAS; i += 128) sBias[i] = __ldg(packB + i);
               tc05::named_sync(3, 128);
@@ -842,17 +843,6 @@ mlp_kernel(const Params p)
           }
           for (int s = 0; s < SL; s++, n++) {
               if (ESTOP && s >= 2 && s >= sStop[it & 1]) break;
-              // weight loads (thread 0): stage pq - q0 of this step's table (sWalk), ring index pq
-              const uint32_t q0 = q;
-              uint32_t pq = q;
-              auto produce = [&](uint32_t upto) {
-                  for (; pq < upto && pq - q0 < (uint32_t)kStepStages; pq++) {
-                      const uint32_t e = sWalk[pq - q0], bytes = (e >> 16) << 11, slot = pq & 3u;
-                      tc05::mbar_arrive_expect_tx(&bars[B_WFULL + slot], bytes);
-                      tc05::bulk_g2s(sRing + slot * kSlot, pack + ((e & 0xffffu) << 11), bytes, &bars[B_WFULL + slot]);
-                  }
-              };
-              if (t == 0) produce(q + 4);
 #pragma unroll 1
               for (int l = 0; l < NL; l++) {
                   const uint32_t g = n * NL + l, buf = g & 1u;
@@ -908,13 +898,11 @@ mlp_kernel(const Params p)
                       // order as their MMAs complete, reduce into a, start block c + 1's group 0 in b and store a.
                       auto block = [&](float (&a)[32], float (&b)[32], int c) {
                           issue(b, ns0, nsb);
-                          auto release = [&]() {
+                          auto release = [&]() {         // this warp is done with the slot of stage qr
                               ts.lap(kSplitWait);
-                              tc05::named_sync(3, 128);       // every warp is done with the slot
-                              ts.lap(kSplitBarrier);
-                              if (t == 0) produce(qr + 5);
+                              if (lane == 0) tc05::mbar_arrive(&bars[B_WEMPTY + (qr & 3u)]);
                               qr++;
-                              ts.lap(kSplitRefill);
+                              ts.lap(kSplitRelease);
                           };
 #pragma unroll 1
                           for (int k = nsb - 1; k > 0; k--) {
@@ -975,7 +963,7 @@ mlp_kernel(const Params p)
               }
           }
       }
-    } else {
+    } else if (warp < kProducerWarp0) {
         // =========================== GATHER WARPS (layer-0 operand producers) ===========================
         set_maxnreg<kRegsGather>();
         const int gt = tid - kGatherWarp0 * 32;
@@ -1207,6 +1195,49 @@ mlp_kernel(const Params p)
                     store_layer0<X3>(sHhi, sHlo, row, half, fh, fl, ext);
                     tc05::fence_proxy_async_smem();
                     tc05::mbar_arrive(&bars[B_FEAT]);
+                }
+            }
+        }
+    } else {
+        // =========================== WEIGHT PRODUCER ===========================
+        // One thread keeps the weight ring full, so that no MMA warp waits for a refill: every stage of a step's table (sWalk),
+        // in order, goes to ring slot q & 3 once the four MMA warps have released the slot's previous stage (B_WEMPTY), with
+        // expect_tx and one bulk copy onto B_WFULL.  It walks the MMA warpgroup's work and step loops and issues exactly the
+        // stages that warpgroup consumes, so no copy is in flight when the CTA exits.
+        set_maxnreg<kRegsProd>();
+        if (warp == kProducerWarp0 && elect_one()) {
+            uint32_t n = 0, q = 0;                                    // global step counter, ring stages issued
+            uint32_t waited = 0;                                      // (timeline build) cycles in empty-barrier waits of step n
+            auto wait_empty = [&]() {
+                if (q < 4) return;                                    // the ring starts empty
+                const uint32_t c = SDB_CLOCK();
+                tc05::mbar_wait(&bars[B_WEMPTY + (q & 3u)], ((q >> 2) - 1) & 1u);
+                waited += SDB_CLOCK() - c;
+            };
+            for (int it = 0;; it++) {
+                const int work = fetch_work(it);
+                if (work < 0) break;
+                const int tile = RAYQ ? 0 : (ONE_STEP ? work : p.tile_list[rec_work(work) / wmult]);
+                const uint8_t *pack = p.pack + (long long)tile_coord(p, tile).img * p.pack_stride;
+                for (int s = 0; s < SL; s++, n++) {
+                    SDB_MARK(3, 1, n, it);
+                    waited = 0;
+                    // The stop test of step s reads what the compositing of step s - 2 decided, so it follows the wait for
+                    // the slot of the step's first stage.  That slot's previous stage is one of the last four of step s - 1,
+                    // all in its colour layer (4 stages or more), and each MMA warp released it after its B_OPND waits of
+                    // step s - 1 (both row blocks, from layer 1 on).  A row block's operand rows of step s - 1 are handed over
+                    // after its compositing of step s - 2.  A later compositing sets sStop to s + 1 or more, which does not
+                    // change the test; the reset for the tile two ahead (gather, after STFREE of this one) comes after the
+                    // MMA warpgroup has run a step of the next tile, whose stages this thread issues after this test.
+                    wait_empty();
+                    if (ESTOP && s >= 2 && s >= sStop[it & 1]) break;
+                    for (int k = 0; k < kStepStages; k++, q++) {
+                        if (k > 0) wait_empty();
+                        const uint32_t e = sWalk[k], bytes = (e >> 16) << 11, slot = q & 3u;
+                        tc05::mbar_arrive_expect_tx(&bars[B_WFULL + slot], bytes);
+                        tc05::bulk_g2s(sRing + slot * kSlot, pack + ((e & 0xffffu) << 11), bytes, &bars[B_WFULL + slot]);
+                    }
+                    SDB_STAMP_PROD(n, waited);
                 }
             }
         }

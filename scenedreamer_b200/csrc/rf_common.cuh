@@ -14,17 +14,19 @@ constexpr int kHidden = 256, kFeat = 128, kOutC = 64, kLevels = 16;
 constexpr int kKExt = 16;                       // extra K columns of the render network's layer 0: labels / fc_1 bias
 constexpr int kMaxM = 8, kMaxS = 64, kMaxLabels = 15;
 constexpr int kEpiThreads = 256, kGatherThreads = 256;
-// warpgroup-aligned roles so that setmaxnreg can move registers between them (here: from the epilogue to the MMA warpgroup):
-//   WG0-1 epilogue (warps 0-7), WG2 MMA + weight loads (warps 8-11), WG3-4 gather (12-19)
-constexpr int kMmaWarp0 = 8, kGatherWarp0 = 12;
-constexpr int kThreads = kEpiThreads + 128 + kGatherThreads;   // 640
-// setmaxnreg can only redistribute the registers the CTA was LAUNCHED with (640 threads x 96 = 61,440; the
-// allocator is a per-CTA pool -- USETMAXREG.TRY_ALLOC.CTAPOOL spins forever otherwise):
-//   8 epilogue warps x 80 + 4 control warps x 112 + 8 gather warps x 104 = 61,440
+// warpgroup-aligned roles so that setmaxnreg can move registers between them (here: from the epilogue, the gather and the
+// producer to the MMA warpgroup):
+//   WG0-1 epilogue (warps 0-7), WG2 MMA (warps 8-11), WG3-4 gather (12-19), WG5 weight-ring producer (20-23)
+constexpr int kMmaWarp0 = 8, kGatherWarp0 = 12, kProducerWarp0 = 20;
+constexpr int kThreads = kEpiThreads + 128 + kGatherThreads + 128;   // 768
+// setmaxnreg can only redistribute the registers the CTA was LAUNCHED with (768 threads x 80 = 61,440, the most ptxas
+// grants a 768-thread __launch_bounds__; the allocator is a per-CTA pool -- USETMAXREG.TRY_ALLOC.CTAPOOL spins forever
+// otherwise):
+//   8 epilogue warps x 72 + 4 MMA warps x 112 + 8 gather warps x 96 + 4 producer warps x 32 = 61,440
 // (the MMA warpgroup holds two 32-register accumulator sets of 64-column blocks and its loop state; at 96 that state spills
 // inside the stage loop)
-constexpr int kRegsLaunch = 96, kRegsEpi = 80, kRegsCtl = 112, kRegsGather = 104;
-static_assert(8 * 32 * kRegsEpi + 4 * 32 * kRegsCtl + 8 * 32 * kRegsGather <= kThreads * kRegsLaunch,
+constexpr int kRegsLaunch = 80, kRegsEpi = 72, kRegsCtl = 112, kRegsGather = 96, kRegsProd = 32;
+static_assert(8 * 32 * kRegsEpi + 4 * 32 * kRegsCtl + 8 * 32 * kRegsGather + 4 * 32 * kRegsProd <= kThreads * kRegsLaunch,
               "setmaxnreg budget exceeds the CTA's launch-time register allocation");
 // a role's register count: released to / taken from the CTA's pool (no instruction when it is the launch count)
 template <int R> __device__ __forceinline__ void set_maxnreg() {
@@ -142,7 +144,7 @@ __host__ __device__ constexpr Smem smem_map(bool x3) {
     m.bars = o; o += 40 * 8;
     m.stop = o; o += 32;                         // early termination: int stop_step[2] (per tile buffer), int vote[2], int voted[2]
     m.sched = o; o += 32;                        // dynamic tile scheduler: int work[4] (ring), int published
-    m.walk = o; o += kMaxStepStages * 4;         // the weight stages of one sample step (read by the MMA warpgroup's thread 0)
+    m.walk = o; o += kMaxStepStages * 4;         // the weight stages of one sample step (read by the producer)
     m.total = o;
     return m;
 }
@@ -156,9 +158,10 @@ constexpr int kStFlags = 2 * kMaxM + 5;      // 1 (uint32: bit0 live, bit1 sky_m
 constexpr int kStFloats = 2 * kMaxM + 6;
 
 // barrier indices.  The MMA warpgroup and the epilogue hand a layer over per 64-row block rb (B_OPND, B_ACC, B_OUTRDY: + rb;
-// B_EPIDONE: + accumulator buffer * 2 + rb), so that one row block's epilogue runs while the other's MMAs do.
+// B_EPIDONE: + accumulator buffer * 2 + rb), so that one row block's epilogue runs while the other's MMAs do.  Ring slot i is
+// loaded (B_WFULL + i, the producer's bulk copy) and free again (B_WEMPTY + i, one arrival per MMA warp).
 enum { B_WFULL = 0, B_FEAT = 4, B_HFREE, B_OPND, B_ACC = B_OPND + 2, B_OUTRDY = B_ACC + 2, B_EPIDONE = B_OUTRDY + 2,
-       B_STRDY = B_EPIDONE + 4, B_STFREE = B_STRDY + 2, B_COMP = B_STFREE + 2, B_COUNT = B_COMP + 1 };
+       B_STRDY = B_EPIDONE + 4, B_STFREE = B_STRDY + 2, B_COMP = B_STFREE + 2, B_WEMPTY = B_COMP + 1, B_COUNT = B_WEMPTY + 4 };
 constexpr int kBarSlots = 40;
 static_assert(B_COUNT <= kBarSlots, "barrier table");
 
@@ -267,11 +270,12 @@ __device__ __forceinline__ void acc_ld(const float *src, float (&v)[NV]) {
 //   layer row 7 = the gather role preparing step n: 0 compositing of step n-2 seen, 1 slots refilled, 2 features gathered, 3 operand buffer free
 // and the MMA warpgroup's row-block time (slot 2 rb -> slot 2 rb + 1) split into cycles spent in kSplit* (thread 0's clock):
 //   debug[kSplitBase + (((n - first) * 8 + layer) * 2 + rb) * 8 + k]
-// full-barrier waits, wgmma issue, wait_group, then what follows wait_group: synchronisation inside the warpgroup (ring-slot
-// release and row-block hand-over), weight refills, the block's sums and bias adds, its accumulator-buffer stores
+// full-barrier waits, wgmma issue, wait_group, then what follows wait_group: the row-block hand-over barrier, ring-slot
+// releases (each warp's empty-barrier arrive), the block's sums and bias adds, its accumulator-buffer stores;
+// and the producer's empty-barrier waits of step n (cycles): debug[kProdBase + n - first]
 constexpr int32_t kTraceMagic = 0x7131;
-constexpr int kTraceSteps = 6, kSplitBase = 512;
-enum { kSplitFull = 0, kSplitIssue, kSplitWait, kSplitBarrier, kSplitRefill, kSplitReduce, kSplitStore, kSplitN };
+constexpr int kTraceSteps = 6, kSplitBase = 512, kProdBase = kSplitBase + kTraceSteps * 8 * 2 * 8;
+enum { kSplitFull = 0, kSplitIssue, kSplitWait, kSplitBarrier, kSplitRelease, kSplitReduce, kSplitStore, kSplitN };
 #ifndef SDB_TIMELINE
 #define SDB_STAMP(n_, layer, slot) do { } while (0)      // compiled out: the stamps cost the epilogue role registers (spills)
 struct TSplit {
@@ -279,7 +283,10 @@ struct TSplit {
     __device__ __forceinline__ void lap(int) {}
 };
 #define SDB_STAMP_SPLIT(n_, layer, rb, ts) do { } while (0)
+#define SDB_STAMP_PROD(n_, cycles) do { } while (0)
+#define SDB_CLOCK() 0u
 #else
+#define SDB_CLOCK() ((uint32_t)clock())
 struct TSplit {                                   // cycles since the last lap, charged to category k
     uint32_t acc[kSplitN], t;
     __device__ __forceinline__ void start() {
@@ -294,6 +301,13 @@ struct TSplit {                                   // cycles since the last lap, 
             const int rel__ = (int)(n_) - p.debug[61];                                                             \
             if (rel__ >= 0 && rel__ < kTraceSteps)                                                                 \
                 for (int k__ = 0; k__ < kSplitN; k__++) p.debug[kSplitBase + ((rel__ * 8 + (layer)) * 2 + (rb)) * 8 + k__] = (int32_t)(ts).acc[k__]; \
+        }                                                                                                          \
+    } while (0)
+#define SDB_STAMP_PROD(n_, cycles)                                                                                 \
+    do {                                                                                                           \
+        if (p.debug != nullptr && blockIdx.x == 0 && p.debug[60] == kTraceMagic) {                                 \
+            const int rel__ = (int)(n_) - p.debug[61];                                                             \
+            if (rel__ >= 0 && rel__ < kTraceSteps) p.debug[kProdBase + rel__] = (int32_t)(cycles);                 \
         }                                                                                                          \
     } while (0)
 #define SDB_STAMP(n_, layer, slot)                                                                                 \

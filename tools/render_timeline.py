@@ -30,6 +30,7 @@ torch.cuda.synchronize()
 L.sdb_debug_set_progress_buffer(ctypes.c_void_p(0))
 t = buf[64:64 + 6 * 8 * 8].cpu().numpy().astype(np.int64).reshape(6, 8, 8) & 0xffffffff
 sp = buf[512:512 + 6 * 8 * 16].cpu().numpy().astype(np.int64).reshape(6, 8, 2, 8)[..., :7]   # rf_common.cuh kSplitBase, kSplit*
+pw = buf[1280:1280 + 6].cpu().numpy().astype(np.int64)                                          # kProdBase: producer's empty waits
 NL = 7
 names = ['fc_1', 'fc_2', 'fc_3', 'fc_4', 'fc_5', 'fc_6', 'out_c']
 
@@ -61,11 +62,13 @@ for s in range(1, 5):
     print('gather for step %d: %s   | MMA layer starts of step %d: %s' % (first + s + 1, [d(g[k], base) for k in range(4)], first + s,
                                                                               [d(t[s, l][0], base) for l in range(NL)]))
 print('step period (MMA warpgroup, fc_1 to fc_1): %s cycles' % [d(t[s + 1, 0][0], t[s, 0][0]) for s in range(0, 5)])
+print('weight producer, empty-barrier waits (the next ring slot not yet released) in steps %d..%d: %s cycles'
+      % (first, first + 4, [int(x) for x in pw[0:5]]))
 print('# MMA warpgroup, where a row block\'s time goes (thread 0, cycles, steps %d..%d averaged): full = full-barrier waits,' % (first + 1, first + 4))
 print('#   issue = wgmma issue + commit, wait = wgmma.wait_group, then what follows wait_group (retire = the sum of the four):')
-print('#   barrier = synchronisation inside the warpgroup (ring-slot release, row-block hand-over), refill = weight-stage refills,')
+print('#   barrier = row-block hand-over barrier, release = ring-slot releases (empty-barrier arrives),')
 print('#   reduce = the block\'s two-group sum and bias adds, store = accumulator-buffer stores')
-cols = ['full', 'issue', 'wait', 'barrier', 'refill', 'reduce', 'store', 'retire', 'sum']
+cols = ['full', 'issue', 'wait', 'barrier', 'release', 'reduce', 'store', 'retire', 'sum']
 print('%-6s %2s %s' % ('layer', 'rb', ' '.join('%7s' % c for c in cols)))
 for l in range(NL):
     m = sp[1:5, l].mean(axis=0)
