@@ -487,7 +487,7 @@ mlp_kernel(const Params p)
             }
             return last;
         };
-        const float *acc_row = p.acc + (size_t)blockIdx.x * 2 * kRows * kHidden + (size_t)row * kHidden;   // accumulator row
+        const float *acc_cta = p.acc + (size_t)blockIdx.x * 2 * kRows * kHidden;   // this CTA's two accumulator buffers (acc_off)
         uint32_t n = 0;                 // global step counter
         int loaded_img = -1;
         for (int it = 0;; it++) {
@@ -546,7 +546,7 @@ mlp_kernel(const Params p)
 #pragma unroll 1
                 for (int l = 0; l < NH; l++) {
                     const uint32_t g = n * NL + l;                   // global layer counter -> accumulator buffer
-                    const float *acc = acc_row + (g & 1u) * kRows * kHidden + half * 128;
+                    const float *acc = acc_cta + (g & 1u) * kRows * kHidden;
                     // kBwd: LeakyReLU sign words of the forward activation A_{6-l} this layer's data gradient passes
                     // through (prefetched before the accumulator wait)
                     uint4 mw = make_uint4(0u, 0u, 0u, 0u);
@@ -568,7 +568,7 @@ mlp_kernel(const Params p)
 #pragma unroll
                         for (int hh = 0; hh < 2; hh++) {
                             float v[16];
-                            acc_ld<16>(acc + c0 + 16 * hh, v);
+                            acc_ld<16>(acc, row, half * 128 + c0 + 16 * hh, v);
                             if constexpr (BWD) {
                                 if (MODE == kBwd && l == 2) {   // dA4 += dsigma * fc_sigma.weight (sigma taps A4, layers.py:115)
                                     const float *ws = sF + kFWsig + half * 128 + c0 + 16 * hh;
@@ -646,7 +646,7 @@ mlp_kernel(const Params p)
 #pragma unroll 1
                     for (int c0 = 0; c0 < 128; c0 += 32) {
                         float v[32];
-                        acc_ld<32>(acc_row + (go & 1u) * kRows * kHidden + half * 128 + c0, v);
+                        acc_ld<32>(acc_cta + (go & 1u) * kRows * kHidden, row, half * 128 + c0, v);
                         const uint32_t word = c0 == 0 ? mw.x : (c0 == 32 ? mw.y : (c0 == 64 ? mw.z : mw.w));
 #pragma unroll
                         for (int j = 0; j < 32; j++) v[j] = ((word >> j) & 1u) ? v[j] : 0.2f * v[j];
@@ -662,11 +662,11 @@ mlp_kernel(const Params p)
                     continue;
                 }
                 float c[32];
-                acc_ld<32>(acc_row + (go & 1u) * kRows * kHidden + half * (BWD ? 64 : 32), c);
+                acc_ld<32>(acc_cta + (go & 1u) * kRows * kHidden, row, half * (BWD ? 64 : 32), c);
                 if constexpr (BWD) {
                     // d(hash-grid features) [128 rays x 128]: this half owns 64 columns -> fp32 record for the table backward
                     float c2[32];
-                    acc_ld<32>(acc_row + (go & 1u) * kRows * kHidden + half * 64 + 32, c2);
+                    acc_ld<32>(acc_cta + (go & 1u) * kRows * kHidden, row, half * 64 + 32, c2);
                     tc05::mbar_arrive(&bars[B_EPIDONE + (go & 1u) * 2 + rb]);
                     if (rb_lead) SDB_STAMP(n, NH, 5 + 2 * rb);
                     float *dst = p.tr.dx0 + slot * kFeat + half * 64;
@@ -862,9 +862,9 @@ mlp_kernel(const Params p)
                       if (t == 0) SDB_STAMP(n, l, 2 * rb);
                       TSplit ts;
                       ts.start();
-                      // element offset of these rows in the accumulator buffers (p.acc is re-read at the store: a 64-bit pointer
-                      // held across the block loop would not fit the registers next to the two accumulator sets)
-                      const uint32_t dst = ((blockIdx.x * 2 + buf) * kRows + rb * 64) * kHidden;
+                      // element offset of this row block in the accumulator buffers (p.acc is re-read at the store: a 64-bit
+                      // pointer held across the block loop would not fit the registers next to the two accumulator sets)
+                      const uint32_t dst = (blockIdx.x * 2 + buf) * kRows * kHidden + acc_off(rb * 64, 0);
                       float x[32], y[32];
                       // issue the MMAs of stages [js0, js1) of the current block into d, one commit group per stage; the first
                       // slab of stage js0 starts a fresh sum (js0 = the first stage of a numerics group)
@@ -933,10 +933,14 @@ mlp_kernel(const Params p)
                           ts.lap(kSplitReduce);
                           if (c + 1 < ncb) issue(b, 0, ns0);
 #ifndef SDB_AB_NO_ACC
+                          // in the buffer's layout (acc_off) a warp's 8-byte stores of one (j, h) fragment pair are two whole
+                          // 128-byte lines: 8 rows of two 4-column chunks, where the row-major buffer took 8 partial lines.  Pair
+                          // (j, h) of the thread sits 8 j columns (two chunks: 128 floats) and 8 h rows (32 floats) past its pair
+                          // (0, 0), so the 16 stores share one address
+                          float *out = p.acc + (dst + (uint32_t)c * 4096u + acc_off(tc05::frag_row(ft, 0), tc05::frag_col(ft, 0)));
 #pragma unroll
                           for (int i = 0; i < 32; i += 2)
-                              *reinterpret_cast<float2 *>(p.acc + (dst + (uint32_t)(tc05::frag_row(ft, i) * kHidden + c * 64 + tc05::frag_col(ft, i)))) =
-                                  make_float2(a[i], a[i + 1]);
+                              *reinterpret_cast<float2 *>(out + (i >> 2) * 128 + ((i >> 1) & 1) * 32) = make_float2(a[i], a[i + 1]);
 #endif
                           ts.lap(kSplitStore);
                       };

@@ -231,24 +231,42 @@ struct Params {
     float *sky_partial;            // [n_tiles, 64] per-tile column sums (deterministic mean)
     int32_t *debug;                // optional host-mapped progress buffer (diagnostics), else nullptr
     TrainBuf tr;                   // training record (TRAIN forward writes it, the kBwd chain reads it)
-    float *acc;                    // [grid][2][128][256] fp32 accumulator buffers, set by the launcher
+    float *acc;                    // [grid][2] fp32 accumulator buffers of 128 x 256 (acc_off), set by the launcher
     const int32_t *view;           // kBwd over one image of a multi-view record: {first live-list position, live tiles} (device)
 };
 
-// NV consecutive fp32 accumulators of one row (written by the MMA warpgroup of the same CTA: plain loads, not the
-// non-coherent path)
+// Element (row, col) of one 128 x 256 fp32 accumulator buffer.  The buffer is 8 blocks of 64 rows x 64 columns, 16 KB each
+// (row block rb, column block cb: block rb * 4 + cb), and a block is stored
+//   [row group r / 16 (4)][column chunk c / 4 (16)][row r % 16 (16)][4 floats]      (r, c inside the block)
+// so that one MMA warp's 16 rows of a block (its part of the wgmma accumulator fragment) are one contiguous 4 KB range, a warp's
+// 8-byte fragment stores of one (j, h) pair fill two whole 128-byte lines (8 rows of two 4-column chunks), and the 32
+// consecutive rows that an epilogue warp reads of one 4-column chunk are two 256-byte runs: 4 lines per 128-bit warp load.
+// In a row-major buffer the same store touched 8 lines and the same load 32.
+__host__ __device__ __forceinline__ constexpr uint32_t acc_off(uint32_t row, uint32_t col) {
+    return (((row >> 6) * (kHidden / 64) + (col >> 6)) << 12) + (((row >> 4) & 3u) << 10) + (((col >> 2) & 15u) << 6) +
+           ((row & 15u) << 2) + (col & 3u);
+}
+static_assert(acc_off(kRows - 1, kHidden - 1) == kRows * kHidden - 1 && acc_off(16, 0) - acc_off(0, 0) == 1024,
+              "accumulator buffer layout");
+
+// Columns col .. col + NV - 1 of one row of an accumulator buffer (col a multiple of NV, so they lie in one 64-column block).
+// Written by the MMA warpgroup of the same CTA; read at L2 (.cg), since every line a warp load touches is used whole by that
+// one instruction and keeping it in L1 would buy nothing.
 // SDB_AB_NO_ACC (diagnostics build only, results are wrong): the accumulator buffer is neither written nor read, so that
 // the kernel time with and without that traffic can be compared on the same work (bench.py --no-early-stop).
 template <int NV>
-__device__ __forceinline__ void acc_ld(const float *src, float (&v)[NV]) {
+__device__ __forceinline__ void acc_ld(const float *buf, int row, int col, float (&v)[NV]) {
+    static_assert(NV % 4 == 0 && NV <= 64 && 64 % NV == 0, "one 64-column block, whole float4s");
 #ifdef SDB_AB_NO_ACC
 #pragma unroll
-    for (int i = 0; i < NV; i++) v[i] = __int_as_float((int)(reinterpret_cast<uintptr_t>(src) & 1));   // 0.0f, not a constant
+    for (int i = 0; i < NV; i++) v[i] = __int_as_float((int)(reinterpret_cast<uintptr_t>(buf) & 1));   // 0.0f, not a constant
+    (void)row; (void)col;
     return;
 #endif
+    const float *src = buf + acc_off(row, col);
 #pragma unroll
     for (int i = 0; i < NV; i += 4) {
-        const float4 a = *reinterpret_cast<const float4 *>(src + i);
+        const float4 a = __ldcg(reinterpret_cast<const float4 *>(src + acc_off(0, i)));   // the next 4-column chunk
         v[i] = a.x; v[i + 1] = a.y; v[i + 2] = a.z; v[i + 3] = a.w;
     }
 }
