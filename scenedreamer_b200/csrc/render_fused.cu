@@ -21,10 +21,11 @@
 //     while the MLP of the current one runs; results wait in registers until the operand buffer is free),
 //     one producer warpgroup (one thread streams the weights into a 4-slot ring with 1-D bulk TMA copies);
 //   * accumulators: a layer's fp32 [128 x 256] result (128 KB) fits neither next to the operand buffers in
-//     shared memory nor in the registers the three roles share, so the MMA warpgroup writes it to a
-//     per-CTA buffer pair in global memory (L2-resident, ping-pong by layer parity) and the epilogue reads
-//     its rows from there; MMA and epilogue hand a layer over per 64-row block, so the epilogue of one row block
-//     runs while the MMAs of the other do;
+//     shared memory nor in the registers the three roles share.  The column blocks that finish after the
+//     layer's MMAs have read their operand columns are staged there in fp32 (half of a hidden layer, all of
+//     the last; hand_plan), the others go to a per-CTA buffer pair in global memory (L2-resident, ping-pong
+//     by layer parity), and the epilogue reads its rows from either; MMA and epilogue hand a layer over per
+//     64-row block, so the epilogue of one row block runs while the MMAs of the other do;
 //   * fc_1's bias and the label embedding ride in layer 0's GEMM: its operand has 16 extra K columns
 //     (one-hot label + constant 1), the weight image carries bias / embedding rows there -- exactly
 //     the reference's fc_m_a(onehot) product; the biases of the later layers (style beta included) are
@@ -350,7 +351,7 @@ mlp_kernel(const Params p)
     static_assert(!BWD || PREC == 1, "the gradient chains run in the range-safe bf16x3 mode");
     constexpr bool X3 = PREC != 0;
     constexpr bool BF16 = PREC == 1;
-    constexpr Smem SM = smem_map(X3);
+    constexpr Smem SM = smem_map();
     constexpr int PARTS = X3 ? 2 : 1;
     constexpr int NH = Net<MODE>::NH, NL = Net<MODE>::NL;
     static_assert(SM.total <= 232448, "shared memory map exceeds the 227 KB a CTA can have");
@@ -371,6 +372,11 @@ mlp_kernel(const Params p)
     constexpr uint32_t kSlot = 16384, kSlabB = 2048 * PARTS;       // ring slot; one k16 slab of a 64-column block
     constexpr int kSps = kSlot / kSlabB;                           // slabs per ring slot
     constexpr int kStepStages = step_stages<MODE>(kSps);
+    // the column-block walk of layer 0, of a hidden layer and of the last layer, and where the epilogue finds each block
+    // (hand_plan)
+    constexpr uint32_t kWalk0 = hand_plan<MODE>(0).walk, kWalkH = hand_plan<MODE>(1).walk, kWalkL = hand_plan<MODE>(NL - 1).walk;
+    constexpr uint32_t kSrc0 = hand_plan<MODE>(0).src, kSrcH = hand_plan<MODE>(1).src, kSrcL = hand_plan<MODE>(NL - 1).src;
+    static_assert(SKYBWD || hand_all_staged<MODE>(NL - 1), "the epilogue reads the last layer from the operand buffer only");
     // Early termination (north star: "early termination"; inference render only).  stop_step[buf] = number of sample
     // steps the tile in state buffer `buf` executes (S until decided).  The epilogue decides during the compositing of
     // step s ("every live ray has transmittance < early_T") and sets s + 2: by the time ANY role starts step s + 2 it
@@ -421,21 +427,24 @@ mlp_kernel(const Params p)
         tc05::mbar_init(&bars[B_COMP], kEpiThreads);
         for (int i = 0; i < 4; i++) tc05::mbar_init(&bars[B_WEMPTY + i], 4);
         tc05::fence_mbar_init();
-        // the ring stages of one sample step, the same for every step and image: per layer and row block, the layer's bytes in
-        // pack order (the pack is stored in streaming order, wpack_off) cut at stage boundaries.  Entry = pack offset / 2 KB |
-        // bytes / 2 KB << 16, so that a refill is one shared load (walking the layers per refill took most of its time).
+        // the ring stages of one sample step, the same for every step and image: per layer and row block, the layer's column
+        // blocks in the order the MMA warpgroup walks them (hand_plan), each block's bytes (contiguous in the pack, wpack_off)
+        // cut at stage boundaries.  Entry = pack offset / 2 KB | bytes / 2 KB << 16, so that a refill is one shared load
+        // (walking the layers per refill took most of its time).
         int k = 0;
         for (int l = 0; l < NL; l++) {
             const int nK = layerK<MODE>(l) / 16, ncb = layerN<MODE>(l) / 64, nsb = block_stages(nK, kSps);
-            for (int rb = 0; rb < 2; rb++) {
-                uint32_t po = (uint32_t)layerOff<MODE>(l, PARTS);    // the layer again for each row block
-                for (int c = 0; c < ncb; c++)
+            const uint32_t walk = l == 0 ? kWalk0 : (l == NL - 1 ? kWalkL : kWalkH);
+            for (int rb = 0; rb < 2; rb++)
+                for (int pos = 0; pos < ncb; pos++) {
+                    const int c = (walk >> (8 * pos)) & 3u;
+                    uint32_t po = (uint32_t)(layerOff<MODE>(l, PARTS) + (int64_t)c * nK * kSlabB);
                     for (int js = 0; js < nsb; js++) {
                         const uint32_t bytes = (uint32_t)stage_slabs(nK, kSps, js) * kSlabB;
                         sWalk[k++] = (po >> 11) | ((bytes >> 11) << 16);
                         po += bytes;
                     }
-            }
+                }
         }
     }
     if (tid < 2) { sStop[tid] = RAYQ ? 0x7fffffff : kMaxS + 1; sVote[tid] = 0; sVoted[tid] = 0; }
@@ -487,7 +496,7 @@ mlp_kernel(const Params p)
             }
             return last;
         };
-        const float *acc_cta = p.acc + (size_t)blockIdx.x * 2 * kRows * kHidden;   // this CTA's two accumulator buffers (acc_off)
+        const float *acc_cta = p.acc + (size_t)blockIdx.x * 2 * kRows * kAccCols;  // this CTA's two accumulator buffers (acc_off)
         uint32_t n = 0;                 // global step counter
         int loaded_img = -1;
         for (int it = 0;; it++) {
@@ -546,7 +555,9 @@ mlp_kernel(const Params p)
 #pragma unroll 1
                 for (int l = 0; l < NH; l++) {
                     const uint32_t g = n * NL + l;                   // global layer counter -> accumulator buffer
-                    const float *acc = acc_cta + (g & 1u) * kRows * kHidden;
+                    const float *acc = acc_cta + (g & 1u) * kRows * kAccCols;
+                    // the column blocks of this layer that the MMA warpgroup staged in the operand buffer, in place (hand_plan)
+                    const uint32_t hsrc = l == 0 ? kSrc0 : kSrcH;
                     // kBwd: LeakyReLU sign words of the forward activation A_{6-l} this layer's data gradient passes
                     // through (prefetched before the accumulator wait)
                     uint4 mw = make_uint4(0u, 0u, 0u, 0u);
@@ -565,10 +576,14 @@ mlp_kernel(const Params p)
                         (void)rec; (void)mword;
                         const uint32_t word = c0 == 0 ? mw.x : (c0 == 32 ? mw.y : (c0 == 64 ? mw.z : mw.w));
                         (void)word;
+                        // one source per 64-column block: the thread's own slots of the operand buffer (read here, then
+                        // overwritten below with the 16-bit operand), or the L2 buffer
+                        const bool staged = (hsrc >> (4 * ((half * 128 + c0) >> 6))) & 15u;
 #pragma unroll
                         for (int hh = 0; hh < 2; hh++) {
                             float v[16];
-                            acc_ld<16>(acc, row, half * 128 + c0 + 16 * hh, v);
+                            if (staged) stg_ld<16>(sHhi, sHlo, row, half * 128 + c0 + 16 * hh, v);
+                            else acc_ld<16>(acc, row, half * 128 + c0 + 16 * hh, v);
                             if constexpr (BWD) {
                                 if (MODE == kBwd && l == 2) {   // dA4 += dsigma * fc_sigma.weight (sigma taps A4, layers.py:115)
                                     const float *ws = sF + kFWsig + half * 128 + c0 + 16 * hh;
@@ -646,7 +661,10 @@ mlp_kernel(const Params p)
 #pragma unroll 1
                     for (int c0 = 0; c0 < 128; c0 += 32) {
                         float v[32];
-                        acc_ld<32>(acc_cta + (go & 1u) * kRows * kHidden, row, half * 128 + c0, v);
+                        const int col = half * 128 + c0;
+                        const uint32_t src = (kSrcL >> (4 * (col >> 6))) & 15u;
+                        if (src) stg_ld<32>(sHhi, sHlo, row, 64 * (int)(src - 1) + (col & 63), v);
+                        else acc_ld<32>(acc_cta + (go & 1u) * kRows * kAccCols, row, col, v);
                         const uint32_t word = c0 == 0 ? mw.x : (c0 == 32 ? mw.y : (c0 == 64 ? mw.z : mw.w));
 #pragma unroll
                         for (int j = 0; j < 32; j++) v[j] = ((word >> j) & 1u) ? v[j] : 0.2f * v[j];
@@ -661,12 +679,15 @@ mlp_kernel(const Params p)
                     if (rb_lead) SDB_STAMP(n, NH, 5 + 2 * rb);
                     continue;
                 }
+                // the last layer is staged whole, clear of the gather's columns (hand_plan): colour block 0 at region 3 (this half's
+                // 32 columns), kBwd block `half` (this half's 64 columns) at its region
                 float c[32];
-                acc_ld<32>(acc_cta + (go & 1u) * kRows * kHidden, row, half * (BWD ? 64 : 32), c);
+                const int ccol = BWD ? 64 * (int)(((kSrcL >> (4 * half)) & 15u) - 1) : 64 * (int)((kSrcL & 15u) - 1) + half * 32;
+                stg_ld<32>(sHhi, sHlo, row, ccol, c);
                 if constexpr (BWD) {
                     // d(hash-grid features) [128 rays x 128]: this half owns 64 columns -> fp32 record for the table backward
                     float c2[32];
-                    acc_ld<32>(acc_cta + (go & 1u) * kRows * kHidden, row, half * 64 + 32, c2);
+                    stg_ld<32>(sHhi, sHlo, row, ccol + 32, c2);
                     tc05::mbar_arrive(&bars[B_EPIDONE + (go & 1u) * 2 + rb]);
                     if (rb_lead) SDB_STAMP(n, NH, 5 + 2 * rb);
                     float *dst = p.tr.dx0 + slot * kFeat + half * 64;
@@ -806,8 +827,9 @@ mlp_kernel(const Params p)
       set_maxnreg<kRegsCtl>();
       // =========================== MMA WARPGROUP ===========================
       // Layer l of a sample step: D[128 x N] = H[128 x K] * W_l^T, one 64-row block rb after the other, each in 64-column
-      // blocks (the sum over K in registers) written once to this CTA's fp32 accumulator buffer (g & 1) in global memory, where
-      // the epilogue reads its rows.  A row block is handed over as soon as it is written, so the epilogue of one row block runs
+      // blocks (the sum over K in registers) written once -- staged in operand columns no MMA of the layer reads any more, or
+      // else to this CTA's fp32 accumulator buffer (g & 1) in global memory (hand_plan) -- where the epilogue reads its rows.
+      // A row block is handed over as soon as it is written, so the epilogue of one row block runs
       // while the MMAs of the other do.  Weights go through a 4-slot ring of 16 KB stages (4 k16 slabs of one 64-column block
       // at x3, 8 at x1; a hidden-layer block at x3 fills the whole ring), one bulk copy each (wpack_off); the producer
       // warpgroup keeps the ring full, the weights are streamed once per row block.  Named barrier 3 is this warpgroup's
@@ -818,10 +840,12 @@ mlp_kernel(const Params p)
       // whole x3 layer that moved the full-frame depth outside its parity bound.  Layers 1 .. NL-1 of the forward networks
       // then add their fp32 bias (the pack's table: hi + lo of the 16-bit parts, what a bias K slab would have summed on the
       // tensor core, exactly) with one more round-to-nearest add.  Two 32-register sets X, Y alternate: block c's group 0 is
-      // in X, its group 1 goes to Y; once both are done X = RN(RN(X + Y) + b), block c + 1's group 0 is issued into Y and X is
-      // stored while it runs, then block c + 1's group 1 goes to X, and so on.  Every stage is its own commit group, so its
-      // ring slot is released (each warp arrives on the slot's empty barrier once its wait_group says the stage's MMAs are
-      // done) and refilled with a stage of the next block by the producer.
+      // in X, its group 1 goes to Y; once both are done X = RN(RN(X + Y) + b), the next block's group 0 is issued into Y and X is
+      // stored while it runs, then the next block's group 1 goes to X, and so on.  A block staged late (kHDelayed) waits for
+      // the next block's group 0 to retire before its store, and that block's group 1 is issued after it.  The blocks are
+      // walked in hand_plan order (a hidden layer: 2, 3, 0, 1); each is the same sum whatever the order.  Every stage is its own
+      // commit group, so its ring slot is released (each warp arrives on the slot's empty barrier once its wait_group says the
+      // stage's MMAs are done) and refilled with a stage of the next block by the producer.
       const int t = tid - kMmaWarp0 * 32;
       static_assert(block_stages(kHidden / 16, kSps) <= 4 && block_stages(kRenderK0 / 16, kSps) <= 4,
                     "the stages of one column block fit the 4-slot ring");
@@ -864,7 +888,8 @@ mlp_kernel(const Params p)
                       ts.start();
                       // element offset of this row block in the accumulator buffers (p.acc is re-read at the store: a 64-bit
                       // pointer held across the block loop would not fit the registers next to the two accumulator sets)
-                      const uint32_t dst = (blockIdx.x * 2 + buf) * kRows * kHidden + acc_off(rb * 64, 0);
+                      const uint32_t dst = (blockIdx.x * 2 + buf) * kRows * kAccCols + acc_off(rb * 64, 0);
+                      const uint32_t walk = l == 0 ? kWalk0 : (l == NL - 1 ? kWalkL : kWalkH);
                       float x[32], y[32];
                       // issue the MMAs of stages [js0, js1) of the current block into d, one commit group per stage; the first
                       // slab of stage js0 starts a fresh sum (js0 = the first stage of a numerics group)
@@ -894,23 +919,33 @@ mlp_kernel(const Params p)
                               ts.lap(kSplitIssue);
                           }
                       };
-                      // block c: its group 0 is in flight in a.  Issue group 1 into b, release the block's ring slots in stage
-                      // order as their MMAs complete, reduce into a, start block c + 1's group 0 in b and store a.
-                      auto block = [&](float (&a)[32], float (&b)[32], int c) {
-                          issue(b, ns0, nsb);
-                          auto release = [&]() {         // this warp is done with the slot of stage qr
+                      // wait for the `pending` stages in flight, oldest first; this warp is done with a stage's ring slot as
+                      // soon as its MMAs are
+                      auto retire = [&](int pending) {
+                          auto release = [&]() {
                               ts.lap(kSplitWait);
                               if (lane == 0) tc05::mbar_arrive(&bars[B_WEMPTY + (qr & 3u)]);
                               qr++;
                               ts.lap(kSplitRelease);
                           };
 #pragma unroll 1
-                          for (int k = nsb - 1; k > 0; k--) {
+                          for (int k = pending - 1; k > 0; k--) {
                               tc05::wgmma_wait_n(k);
                               release();
                           }
+                          // always: ptxas serialises every wgmma of the kernel if one path may read an accumulator set in flight
                           tc05::wgmma_wait<0>();
-                          release();
+                          if (pending > 0) release();
+                      };
+                      bool g0_done = false;          // the current block's group 0 has retired (the block before it was staged late)
+                      // the pos-th block of the walk: its group 0 is in flight in a.  Issue group 1 into b, retire the block's
+                      // stages, reduce into a, start the next block's group 0 in b and store a.
+                      auto block = [&](float (&a)[32], float (&b)[32], int pos) {
+                          const uint32_t w = walk >> (8 * pos);
+                          const int c = (int)(w & 3u);
+                          issue(b, ns0, nsb);
+                          retire(g0_done ? nsb - ns0 : nsb);
+                          g0_done = false;
                           tc05::wgmma_fence_acc(a);
                           tc05::wgmma_fence_acc(b);
                           if (nsb > ns0) {
@@ -931,24 +966,48 @@ mlp_kernel(const Params p)
                               }
                           }
                           ts.lap(kSplitReduce);
-                          if (c + 1 < ncb) issue(b, 0, ns0);
+                          if (pos + 1 < ncb) issue(b, 0, ns0);
+                          if (!(w & kHStaged)) {
 #ifndef SDB_AB_NO_ACC
-                          // in the buffer's layout (acc_off) a warp's 8-byte stores of one (j, h) fragment pair are two whole
-                          // 128-byte lines: 8 rows of two 4-column chunks, where the row-major buffer took 8 partial lines.  Pair
-                          // (j, h) of the thread sits 8 j columns (two chunks: 128 floats) and 8 h rows (32 floats) past its pair
-                          // (0, 0), so the 16 stores share one address
-                          float *out = p.acc + (dst + (uint32_t)c * 4096u + acc_off(tc05::frag_row(ft, 0), tc05::frag_col(ft, 0)));
+                              // in the buffer's layout (acc_off) a warp's 8-byte stores of one (j, h) fragment pair are two whole
+                              // 128-byte lines: 8 rows of two 4-column chunks, where the row-major buffer took 8 partial lines.
+                              // Pair (j, h) of the thread sits 8 j columns (two chunks: 128 floats) and 8 h rows (32 floats) past
+                              // its pair (0, 0), so the 16 stores share one address
+                              float *out = p.acc + (dst + (uint32_t)(c & 1) * 4096u + acc_off(tc05::frag_row(ft, 0), tc05::frag_col(ft, 0)));
 #pragma unroll
-                          for (int i = 0; i < 32; i += 2)
-                              *reinterpret_cast<float2 *>(out + (i >> 2) * 128 + ((i >> 1) & 1) * 32) = make_float2(a[i], a[i + 1]);
+                              for (int i = 0; i < 32; i += 2)
+                                  *reinterpret_cast<float2 *>(out + (i >> 2) * 128 + ((i >> 1) & 1) * 32) = make_float2(a[i], a[i + 1]);
 #endif
+                          } else {
+                              // Staged in operand region r of this row block's rows.  The stores overwrite operand rows this
+                              // warpgroup's wgmma read: every MMA that reads the region has retired in this warp (wait_group), and
+                              // with kHBarrier the four warps meet first, so no warp's MMAs still read it -- no warp relies on
+                              // another reading only its own 16 A rows.
+                              if (w & kHDelayed) {
+                                  retire(ns0);        // the next block's group 0, the region's last reader
+                                  g0_done = true;
+                              }
+                              // layer 0 may stage in the region where the last layer of step n - 1 left its output (and its
+                              // epilogue overwrites those rows): the epilogue of that layer has read both halves first
+                              if (l == 0 && (w & kHFirst) && g >= 1)
+                                  tc05::mbar_wait(&bars[B_EPIDONE + ((g - 1) & 1u) * 2 + rb], ((g - 1) >> 1) & 1u);
+                              if (w & kHBarrier) tc05::named_sync(3, 128);
+                              // pair (j, h) of chunk 8 r + j, row 16 warp + lane / 4 + 8 h: lanes 0-1 of a quad hold its floats
+                              // 0-3 (hi slot), lanes 2-3 its floats 4-7 (lo slot), so 8 rows of a quad column are 128
+                              // contiguous bytes of either part: conflict-free 8-byte stores
+                              const uint32_t sa = tc05::smem_u32(smem) + ((ft & 2u) ? SM.h_lo : SM.h_hi) + (ft & 1u) * 8u +
+                                                  tc05::chunk_off(kRows, rb * 64 + tc05::frag_row(ft, 0), 8u * ((w >> 4) & 3u));
+#pragma unroll
+                              for (int i = 0; i < 32; i += 2)
+                                  tc05::st_shared_v2f(sa + (i >> 2) * kRows * 16 + ((i >> 1) & 1) * 128, a[i], a[i + 1]);
+                          }
                           ts.lap(kSplitStore);
                       };
                       issue(x, 0, ns0);
 #pragma unroll 1
-                      for (int c = 0; c < ncb; c += 2) {
-                          block(x, y, c);
-                          if (c + 1 < ncb) block(y, x, c + 1);
+                      for (int pos = 0; pos < ncb; pos += 2) {
+                          block(x, y, pos);
+                          if (pos + 1 < ncb) block(y, x, pos + 1);
                       }
                       __threadfence_block();
                       tc05::named_sync(3, 128);
@@ -1507,7 +1566,7 @@ int launch_pack(const float *w0, const float *b0, const float *emb, int n_labels
     return SDB_OK;
 }
 
-// Per-CTA fp32 accumulator buffers of the fused kernels ([grid][2][128][256], L2-resident), one per (device, stream): launches
+// Per-CTA fp32 accumulator buffers of the fused kernels ([grid][2][128][128], L2-resident), one per (device, stream): launches
 // on one stream are ordered, so they can share it; launches on different streams get different buffers.  A buffer is
 // allocated (or grown) on the first launch that needs it and kept for the life of the process.  Allocation is refused while
 // the stream is being captured into a CUDA graph: run one launch of the same size outside the capture first.
@@ -1524,7 +1583,7 @@ static int acc_buffers(int grid, cudaStream_t st, float **out) {
         if (cs != cudaStreamCaptureStatusNone) return SDB_EUNSUPPORTED;
         if (b.first) SDB_CUDA(cudaFree(b.first));
         b = std::make_pair((float *)nullptr, 0);
-        SDB_CUDA(cudaMalloc(&b.first, (size_t)grid * 2 * kRows * kHidden * sizeof(float)));
+        SDB_CUDA(cudaMalloc(&b.first, (size_t)grid * 2 * kRows * kAccCols * sizeof(float)));
         b.second = grid;
     }
     *out = b.first;
@@ -1536,7 +1595,7 @@ int launch_mlp(const Params &p_in, int grid, cudaStream_t st) {
     Params p = p_in;
     const int e = acc_buffers(grid, st, &p.acc);
     if (e != SDB_OK) return e;
-    const size_t smem = smem_map(PREC != 0).total;
+    const size_t smem = smem_map().total;
     cudaFuncAttributes fa;
     SDB_CUDA(cudaFuncGetAttributes(&fa, mlp_kernel<PREC, RAW5D, MODE, TRAIN, RAYQ, GU>));
     if (fa.numRegs < kRegsLaunch) return SDB_EUNSUPPORTED;   // setmaxnreg pool would be too small: refuse rather than hang

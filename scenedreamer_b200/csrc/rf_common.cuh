@@ -129,11 +129,11 @@ __device__ __forceinline__ bool elect_one() {
 struct Smem {
     uint32_t h_hi, h_lo, ring, fsec, bias, scales, frac, sig, state, bars, stop, sched, walk, total;
 };
-__host__ __device__ constexpr Smem smem_map(bool x3) {
+__host__ __device__ constexpr Smem smem_map() {
     Smem m{};
     uint32_t o = 0;
     m.h_hi = o; o += kHBytes;
-    m.h_lo = o; if (x3) o += kHBytes;
+    m.h_lo = o; o += kHBytes;                   // fp16 (!x3): no lo operand, the lo half of blocks staged there (hand_plan)
     m.ring = o; o += kRingBytes;
     m.fsec = o; o += kFTotal * 4;
     m.bias = o; o += Net<kRender>::NBIAS * 4;   // the largest bias table (read by the MMA warpgroup)
@@ -231,23 +231,126 @@ struct Params {
     float *sky_partial;            // [n_tiles, 64] per-tile column sums (deterministic mean)
     int32_t *debug;                // optional host-mapped progress buffer (diagnostics), else nullptr
     TrainBuf tr;                   // training record (TRAIN forward writes it, the kBwd chain reads it)
-    float *acc;                    // [grid][2] fp32 accumulator buffers of 128 x 256 (acc_off), set by the launcher
+    float *acc;                    // [grid][2] fp32 accumulator buffers of 128 x 128 (acc_off), set by the launcher
     const int32_t *view;           // kBwd over one image of a multi-view record: {first live-list position, live tiles} (device)
 };
 
-// Element (row, col) of one 128 x 256 fp32 accumulator buffer.  The buffer is 8 blocks of 64 rows x 64 columns, 16 KB each
-// (row block rb, column block cb: block rb * 4 + cb), and a block is stored
+// ---- layer hand-off: the order of a row block's column blocks, and where each finished block goes ----
+// Block c of a layer is output columns 64c .. 64c+63.  Operand region r of the shared-memory operand buffer is K slabs
+// 4r .. 4r+3 (columns 64r .. 64r+63); a layer reads a slab in numerics group 0 (slabs 0..7) or group 1 (slabs 8..nK-1).  A
+// finished block is STAGED as fp32 in a region of its own rows that no MMA of the layer reads any more, or goes to the per-CTA
+// accumulator buffer in L2 (acc_off).  In a hidden layer the region is the block's own (c): the epilogue turns it into the
+// next layer's operand in place.  The last layer's output only goes to the epilogue, so it may sit in any dead region that
+// the gather does not write -- the gather writes the next step's layer-0 operand (columns 0 .. K0-1) as soon as B_HFREE fires.
+// bit 0: group 0 of layer l reads a slab of region r, bit 1: group 1 does
+template <int MODE> __host__ __device__ constexpr int region_readers(int l, int r) {
+    const int nK = layerK<MODE>(l) / 16, s0 = 4 * r, g0e = nK < 8 ? nK : 8;
+    return (s0 < g0e ? 1 : 0) | (s0 < nK && s0 + 4 > 8 ? 2 : 0);
+}
+// walk, byte p = the p-th column block the MMA warpgroup computes: bits 0-1 the block c, then the flags below and the region
+// (bits 4-5) it is staged in.  src, nibble c: 0 = block c is in the L2 buffer (at column block c & 1), r + 1 = staged in region r.
+enum { kHStaged = 4, kHDelayed = 8, kHBarrier = 64, kHFirst = 128 };
+// kHDelayed: the region is read by the NEXT block's group 0 only; the block stays in its accumulator set until that group has
+//            retired, and the next block's group 1 is issued into the set after the store
+// kHBarrier: an MMA of this layer read the region since the warpgroup last met, so it meets (named barrier 3) before the store
+// kHFirst:   the row block's first staged store
+struct HandPlan { uint32_t walk, src; };
+template <int MODE> __host__ __device__ constexpr HandPlan hand_plan(int l) {
+    const bool last = l == Net<MODE>::NL - 1;
+    const int ncb = layerN<MODE>(l) / 64, L = ncb - 1;
+    // order: blocks whose own region group 1 reads first (they cannot be staged), then those whose region no MMA of the layer
+    // reads, then those only group 0 reads: a hidden layer walks 2, 3, 0, 1.  The last layer walks 0, 1, ...
+    int order[4] = {0, 1, 2, 3}, n = 0;
+    if (!last)
+        for (int cat = 2; cat < 5; cat++)                       // categories 2, 0, 1
+            for (int c = 0; c < ncb; c++)
+                if ((region_readers<MODE>(l, c) & 2 ? 2 : region_readers<MODE>(l, c)) == cat % 3) order[n++] = c;
+    const int r_min = last ? (Net<MODE>::K0 + 63) / 64 : 0;    // the last layer: regions clear of the gather's columns
+    int dst[4] = {-1, -1, -1, -1}, used = 0;
+    bool del[4] = {false, false, false, false};
+    for (int p = 0; p < ncb; p++) {
+        for (int pass = 0; pass < 2 && dst[p] < 0; pass++)     // pass 0: dead once the block is done; pass 1: delayed
+            for (int r = last ? 3 : order[p]; r >= (last ? r_min : order[p]); r--) {
+                const int rd = region_readers<MODE>(l, r);
+                const bool dead = pass == 0 ? (p == L || rd == 0) : (p == L - 1 && rd == 1);
+                if (!(used >> r & 1) && dead) { dst[p] = r; del[p] = pass == 1; used |= 1 << r; break; }
+            }
+    }
+    // when the last reader of each region retires, in the order W(p) = 3p (block p's groups), staged store of block p: 3p + 1,
+    // or 3p + 2 with block p + 1's group 0 retired just before
+    HandPlan h{0u, 0u};
+    int met = -1;
+    for (int p = 0; p < ncb; p++) {
+        uint32_t b = (uint32_t)order[p];
+        if (dst[p] >= 0) {
+            const int rd = region_readers<MODE>(l, dst[p]);
+            const int t_read = rd == 0 ? -1 : ((rd & 2) || L == 0 || !del[L - 1] ? 3 * L : 3 * L - 1);
+            b |= kHStaged | (del[p] ? kHDelayed : 0u) | ((uint32_t)dst[p] << 4) | (h.src == 0 ? kHFirst : 0u);
+            if (t_read > met) { b |= kHBarrier; met = 3 * p + (del[p] ? 2 : 1); }
+            h.src |= (uint32_t)(dst[p] + 1) << (4 * order[p]);
+        }
+        h.walk |= b << (8 * p);
+    }
+    return h;
+}
+template <int MODE> __host__ __device__ constexpr bool hand_all_staged(int l) {
+    for (int c = 0; c < layerN<MODE>(l) / 64; c++)
+        if ((hand_plan<MODE>(l).src >> (4 * c) & 15u) == 0) return false;
+    return true;
+}
+// every mode: at most two blocks of a layer pass through L2, in different column blocks of the buffer; a hidden layer stages a
+// block in its own region; and layer 0 stages a block (its first staged store is where the MMA warpgroup waits until the
+// epilogue has read the previous step's last layer)
+template <int MODE> __host__ __device__ constexpr bool hand_plan_ok() {
+    for (int l = 0; l < Net<MODE>::NL; l++) {
+        const HandPlan h = hand_plan<MODE>(l);
+        int l2 = 0;
+        for (int c = 0; c < layerN<MODE>(l) / 64; c++) {
+            const uint32_t src = h.src >> (4 * c) & 15u;
+            if (src == 0) {
+                if (l2 >> (c & 1) & 1) return false;
+                l2 |= 1 << (c & 1);
+            } else if (l < Net<MODE>::NL - 1 && src != (uint32_t)c + 1) {
+                return false;
+            }
+        }
+        if (l == 0 && h.src == 0) return false;
+    }
+    return true;
+}
+static_assert(hand_plan_ok<kRender>() && hand_plan_ok<kSky>() && hand_plan_ok<kBwd>() && hand_plan_ok<kSkyBwd>(), "hand-off plan");
+static_assert(hand_plan<kRender>(1).walk == 0x15cc0302u && hand_plan<kRender>(1).src == 0x21u, "hidden layer: 2, 3, 0, 1");
+
+// Element (row, col) of one fp32 accumulator buffer: the column blocks of a 128 x 256 layer output that are not staged, at most
+// two per layer, block c at column block c & 1.  The buffer is 4 blocks of 64 rows x 64 columns, 16 KB each (row block rb,
+// column block c: block rb * 2 + (c & 1)), and a block is stored
 //   [row group r / 16 (4)][column chunk c / 4 (16)][row r % 16 (16)][4 floats]      (r, c inside the block)
 // so that one MMA warp's 16 rows of a block (its part of the wgmma accumulator fragment) are one contiguous 4 KB range, a warp's
 // 8-byte fragment stores of one (j, h) pair fill two whole 128-byte lines (8 rows of two 4-column chunks), and the 32
 // consecutive rows that an epilogue warp reads of one 4-column chunk are two 256-byte runs: 4 lines per 128-bit warp load.
 // In a row-major buffer the same store touched 8 lines and the same load 32.
+constexpr int kAccCols = 128;
 __host__ __device__ __forceinline__ constexpr uint32_t acc_off(uint32_t row, uint32_t col) {
-    return (((row >> 6) * (kHidden / 64) + (col >> 6)) << 12) + (((row >> 4) & 3u) << 10) + (((col >> 2) & 15u) << 6) +
+    return (((row >> 6) * (kAccCols / 64) + ((col >> 6) & 1u)) << 12) + (((row >> 4) & 3u) << 10) + (((col >> 2) & 15u) << 6) +
            ((row & 15u) << 2) + (col & 3u);
 }
-static_assert(acc_off(kRows - 1, kHidden - 1) == kRows * kHidden - 1 && acc_off(16, 0) - acc_off(0, 0) == 1024,
+static_assert(acc_off(kRows - 1, kHidden - 1) == kRows * kAccCols - 1 && acc_off(16, 0) - acc_off(0, 0) == 1024,
               "accumulator buffer layout");
+
+// Columns col .. col + NV - 1 of one row of a block staged in the operand buffer (col a multiple of 8): the MMA warpgroup
+// stores floats 0-3 of 8-column chunk j in the hi part's 16-byte slot of (row, j) and floats 4-7 in the lo part's slot.  The
+// epilogue thread that owns the row reads both and writes its 16-bit operand back into the same two slots.
+template <int NV>
+__device__ __forceinline__ void stg_ld(const uint8_t *sHhi, const uint8_t *sHlo, int row, int col, float (&v)[NV]) {
+    static_assert(NV % 8 == 0, "whole 8-column chunks");
+#pragma unroll
+    for (int i = 0; i < NV; i += 8) {
+        const uint32_t off = tc05::chunk_off(kRows, row, (col + i) >> 3);
+        const float4 a = *reinterpret_cast<const float4 *>(sHhi + off), b = *reinterpret_cast<const float4 *>(sHlo + off);
+        v[i] = a.x; v[i + 1] = a.y; v[i + 2] = a.z; v[i + 3] = a.w;
+        v[i + 4] = b.x; v[i + 5] = b.y; v[i + 6] = b.z; v[i + 7] = b.w;
+    }
+}
 
 // Columns col .. col + NV - 1 of one row of an accumulator buffer (col a multiple of NV, so they lie in one 64-column block).
 // Written by the MMA warpgroup of the same CTA; read at L2 (.cg), since every line a warp load touches is used whole by that

@@ -102,6 +102,10 @@ __device__ __forceinline__ void wgmma_fence_acc(float (&d)[R]) {
 #pragma unroll
     for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
+// two floats to shared-memory address `saddr` (8-byte aligned)
+__device__ __forceinline__ void st_shared_v2f(uint32_t saddr, float a, float b) {
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(saddr), "f"(a), "f"(b) : "memory");
+}
 // generic-proxy smem writes -> visible to the async proxy (tensor core / TMA reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
