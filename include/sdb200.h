@@ -450,6 +450,41 @@ int sdb_cnn_backward(int32_t H, int32_t W, const void *d_record, const float *d_
                      void *d_workspace, void *stream);
 
 /* --------------------------------------------------------------------------------------------
+ * f1 under autograd at a chosen precision: the training block above with a `precision` argument, for
+ * mixed-precision training (torch.autocast) as well as the fp32-grade path.
+ *   sdb_cnn_pack_bytes_ex / sdb_cnn_pack_ex take pack precisions 0..3: 0..2 make the same bytes as
+ *   sdb_cnn_pack, 3 = one bf16 plane per weight.
+ *   The training entries take 0 = one fp16 pass, 1 = bf16 hi/lo split x3 (the entries above: every
+ *   _ex call at 1 computes bit for bit what its counterpart does), 3 = one bf16 pass; 2 and anything
+ *   else -> SDB_EUNSUPPORTED (sizes: 0).  At 0 and 3 every product is one 16-bit MMA with fp32
+ *   accumulation, the class of autocast's own fp16 / bf16 convolutions: the record holds ONE plane of
+ *   the forward's type per activation (same order, layout and zero borders; about half the bytes),
+ *   gradients travel as single planes of that type, and the epilogue arithmetic, channel sums and
+ *   dL/d net_out stay fp32.  At 0, rgb and rgb_raw of the training forward equal sdb_cnn_forward's at
+ *   precision 0 on the same pack.  fp16 gradient planes want a scaled loss (GradScaler); bf16 does not.
+ *   Pack, record, backward pack and workspace of one pass must all come from the same precision.
+ *   sdb_cnn_debug_record_layout_ex: the 14 int64 of sdb_cnn_debug_record_layout at that precision.
+ * Argument checks: NULL pointers and H, W <= 0 -> SDB_EINVAL before the precision is looked at.
+ * ------------------------------------------------------------------------------------------ */
+int64_t sdb_cnn_pack_bytes_ex(int32_t precision);
+int sdb_cnn_pack_ex(const float *d_w1, const float *d_b1, const float *d_w2a, const float *d_b2a, const float *d_w2b,
+                    const float *d_w3a, const float *d_b3a, const float *d_w3b, const float *d_w4a, const float *d_b4a,
+                    const float *d_w4b, const float *d_b4b, const float *d_w4, const float *d_b4, int32_t precision,
+                    void *d_pack, void *stream);
+int64_t sdb_cnn_train_record_bytes_ex(int32_t H, int32_t W, int32_t precision);
+int sdb_cnn_train_forward_ex(const float *d_net_out, int32_t H, int32_t W, const void *d_pack, const float *d_mod,
+                             int32_t precision, float *d_rgb, float *d_rgb_raw, void *d_record, void *stream);
+int64_t sdb_cnn_backward_pack_bytes_ex(int32_t precision);
+int sdb_cnn_pack_backward_ex(const float *d_w1, const float *d_w2a, const float *d_w2b, const float *d_w3a,
+                             const float *d_w3b, const float *d_w4a, const float *d_w4b, int32_t precision, void *d_pack,
+                             void *stream);
+int64_t sdb_cnn_backward_workspace_bytes_ex(int32_t H, int32_t W, int32_t precision);
+int sdb_cnn_backward_ex(int32_t H, int32_t W, int32_t precision, const void *d_record, const float *d_grad_rgb,
+                        const float *d_grad_rgb_raw, const void *d_bwd_pack, const void *d_pack, const float *d_mod,
+                        const sdb_cnn_grads *g, void *d_workspace, void *stream);
+int sdb_cnn_debug_record_layout_ex(int32_t H, int32_t W, int32_t precision, int64_t *out);
+
+/* --------------------------------------------------------------------------------------------
  * a8 (training): the style modulation of LightningMLP's five ModLinear layers for ONE style code, folded into plain
  * weights, forward and backward (imaginaire/model_utils/layers.py:241-271 as used at :92-126):
  *   alpha = weight_alpha z + bias_alpha [I], beta = weight_beta z + bias_beta [O], W' = W * alpha (per input column).

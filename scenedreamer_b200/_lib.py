@@ -81,6 +81,16 @@ SIGNATURES = {
     'sdb_cnn_backward_workspace_bytes': (c_i64, [c_i32, c_i32]),
     'sdb_cnn_backward': (c_int, [c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                  c_void_p]),
+    'sdb_cnn_pack_bytes_ex': (c_i64, [c_i32]),
+    'sdb_cnn_pack_ex': (c_int, [c_void_p] * 14 + [c_i32, c_void_p, c_void_p]),
+    'sdb_cnn_train_record_bytes_ex': (c_i64, [c_i32, c_i32, c_i32]),
+    'sdb_cnn_train_forward_ex': (c_int, [c_void_p, c_i32, c_i32, c_void_p, c_void_p, c_i32, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'sdb_cnn_backward_pack_bytes_ex': (c_i64, [c_i32]),
+    'sdb_cnn_pack_backward_ex': (c_int, [c_void_p] * 7 + [c_i32, c_void_p, c_void_p]),
+    'sdb_cnn_backward_workspace_bytes_ex': (c_i64, [c_i32, c_i32, c_i32]),
+    'sdb_cnn_backward_ex': (c_int, [c_i32, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, c_void_p]),
+    'sdb_cnn_debug_record_layout_ex': (c_int, [c_i32, c_i32, c_i32, ctypes.POINTER(c_i64)]),
     'sdb_adam_step': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, ctypes.c_double, ctypes.c_double, ctypes.c_double,
                               ctypes.c_double, c_i64, c_void_p]),
     'sdb_pose_stats_workspace_bytes': (c_i64, [c_i32]),

@@ -237,14 +237,16 @@ __device__ __forceinline__ void mma_pass(float (&acc)[2][2][32], const LayerPara
     }
 }
 
-// Forward layer.  <X3, fp16>: inference (precisions 2 and 0).  <true, bf16>: the training forward, which also records the
-// pre-modulation sum u of a modulated layer in the plane pair right before its output (the record layout, RecLayout).
-template <bool X3, bool BF16>
+// Forward layer.  <X3, fp16, false>: inference (precisions 2 and 0).  REC: a training forward, which also records the
+// pre-modulation sum u of a modulated layer in the planes right before its output (the record layout, RecLayout):
+// <true, bf16> the bf16 x3 path, <false, fp16 / bf16> the one-pass paths of autocast.
+template <bool X3, bool BF16, bool REC>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_kernel(const LayerParams p)
 {
+    constexpr int P = X3 ? 2 : 1;
     extern __shared__ __align__(1024) uint8_t smem[];
-    const Smem sm = smem_map(p.taps, X3 ? 2 : 1);
+    const Smem sm = smem_map(p.taps, P);
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem + sm.bars);
     float *sBias = reinterpret_cast<float *>(smem + sm.consts);
     float *sModW = sBias + kCh, *sModB = sModW + kCh, *sW4 = sModB + kCh, *sB4 = sW4 + 3 * kCh;
@@ -306,7 +308,7 @@ conv_kernel(const LayerParams p)
                                     v1 = r.y + v1;
                                 }
                                 if (p.epi == EPI_RES_MOD_LRELU) {
-                                    if (BF16 && valid) store_split2<X3, BF16>(p.out - 2 * out_plane + off, out_plane, v0, v1);   // u: the record's pair before y
+                                    if (REC && valid) store_split2<X3, BF16>(p.out - P * out_plane + off, out_plane, v0, v1);   // u: the record's planes before y
                                     v0 = lrelu(fmaf(v0, sModW[ch], sModB[ch]));
                                     v1 = lrelu(fmaf(v1, sModW[ch + 1], sModB[ch + 1]));
                                 } else if (p.epi == EPI_RES_BIAS_LRELU_RGB) {
@@ -381,6 +383,10 @@ conv_kernel(const LayerParams p)
 //   conv1^T           fp32 NHWC                                       -> dL/dnet_out
 // and after each data step the weight gradient of that layer (conv_wgrad_kernel).  Gradients are bf16 hi/lo plane pairs
 // in the activation layout, zero outside the frame.  Every product is bf16 x3 (hi hi + lo hi + hi lo), fp32 accumulation.
+//
+// One-pass training (X3 = false; precision 0 = fp16, 3 = bf16): the class of autocast's own convolutions.  The same record
+// order and layout with ONE 16-bit plane per activation in the forward's type, single gradient planes in that type, one
+// product per MMA step, fp32 accumulation and the same fp32 epilogue arithmetic everywhere.
 
 // Backward of tanh, conv4 (256 -> 3) and the last LeakyReLU, per pixel; block (., c) owns 8-channel chunk c.  Each of the
 // 32 chunk rows recomputes g_raw from G_rgb, G_raw and rgb (36 B per pixel): those planes are at most 20 MB at 570 x 990 and
@@ -395,6 +401,7 @@ struct HeadParams {
     int H, W, Hp, Wp;
 };
 
+template <bool X3, bool BF16>
 __global__ void __launch_bounds__(256)
 head_bwd_kernel(const HeadParams h)
 {
@@ -424,20 +431,20 @@ head_bwd_kernel(const HeadParams h)
         }
         const size_t off = ((((size_t)(y + 1) * (kCh / 8)) + c) * h.Wp + (x + 1)) * 16;
         float yh[8], yl[8], g[8];
-        unpack8<true>(*reinterpret_cast<const uint4 *>(h.y4 + off), yh);
-        unpack8<true>(*reinterpret_cast<const uint4 *>(h.y4 + plane + off), yl);
+        unpack8<BF16>(*reinterpret_cast<const uint4 *>(h.y4 + off), yh);
+        if (X3) unpack8<BF16>(*reinterpret_cast<const uint4 *>(h.y4 + plane + off), yl);
 #pragma unroll
         for (int j = 0; j < 8; j++) {
             const float gy = fmaf(w[2][j], gr[2], fmaf(w[1][j], gr[1], w[0][j] * gr[0]));
             g[j] = yh[j] > 0.0f ? gy : 0.2f * gy;
             part[24 + j] += g[j];
 #pragma unroll
-            for (int k = 0; k < 3; k++) part[8 * k + j] = fmaf(gr[k], yh[j] + yl[j], part[8 * k + j]);
+            for (int k = 0; k < 3; k++) part[8 * k + j] = fmaf(gr[k], X3 ? yh[j] + yl[j] : yh[j], part[8 * k + j]);
         }
         uint4 hi, lo;
-        split8<true>(g, hi, lo);
+        split8<BF16>(g, hi, lo);
         *reinterpret_cast<uint4 *>(h.out + off) = hi;
-        *reinterpret_cast<uint4 *>(h.out + plane + off) = lo;
+        if (X3) *reinterpret_cast<uint4 *>(h.out + plane + off) = lo;
     }
 #pragma unroll
     for (int i = 0; i < 35; i++) {
@@ -471,12 +478,13 @@ struct BwdParams {
     float *dx;                  // conv1^T: dL/dnet_out [H][W][64] fp32 instead of `out`
 };
 
+template <bool X3, bool BF16>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_bwd_kernel(const BwdParams q)
 {
     extern __shared__ __align__(1024) uint8_t smem[];
     const LayerParams &p = q.l;
-    const Smem sm = smem_map(p.taps, 2);
+    const Smem sm = smem_map(p.taps, X3 ? 2 : 1);
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem + sm.bars);
     float *sScale = reinterpret_cast<float *>(smem + sm.consts), *sSum1 = sScale + kCh, *sSum2 = sSum1 + kCh;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -491,10 +499,10 @@ conv_bwd_kernel(const BwdParams q)
     __syncthreads();
 
     if (warp == 8) {
-        load_slabs<true>(p, smem, sm, bars, lane, n_slabs, n_tiles, taps == 9 ? 4 : 2, taps == 9 ? 0 : 1,
-                         plane_bytes(p.Hp, p.in_chunks, p.Wp));
+        load_slabs<X3>(p, smem, sm, bars, lane, n_slabs, n_tiles, taps == 9 ? 4 : 2, taps == 9 ? 0 : 1,
+                       plane_bytes(p.Hp, p.in_chunks, p.Wp));
     } else if (warp == 9) {
-        load_weights<true>(p, smem, sm, bars, lane, n_slabs, n_tiles, taps);
+        load_weights<X3>(p, smem, sm, bars, lane, n_slabs, n_tiles, taps);
     } else {
         const int o = warp >> 2, t = tid & 127;
         const size_t plane = plane_bytes(p.Hp, kCh / 8, p.Wp);
@@ -504,7 +512,7 @@ conv_bwd_kernel(const BwdParams q)
 #pragma unroll 1
             for (int pass = 0; pass < kPasses; pass++) {
                 float acc[2][2][32];
-                mma_pass<true, true>(acc, p, smem, sm, bars, o, t, pass, taps, n_slabs, scnt, wcnt);
+                mma_pass<X3, BF16>(acc, p, smem, sm, bars, o, t, pass, taps, n_slabs, scnt, wcnt);
 #pragma unroll
                 for (int nh = 0; nh < 2; nh++) {
 #pragma unroll
@@ -520,19 +528,19 @@ conv_bwd_kernel(const BwdParams q)
                                 const size_t off = ((((size_t)(y + 1) * (kCh / 8)) + (ch >> 3)) * p.Wp + (x + 1)) * 16 + (ch & 7) * 2;
                                 float v0 = acc[rb][nh][4 * j + 2 * h], v1 = acc[rb][nh][4 * j + 2 * h + 1];
                                 if (p.res) {
-                                    const float2 r = load_pair<true, true>(p.res + off, plane);
+                                    const float2 r = load_pair<X3, BF16>(p.res + off, plane);
                                     v0 += r.x;
                                     v1 += r.y;
                                 }
                                 if (q.sign) {
-                                    const float2 sg = tc05::unpack2<true>(*reinterpret_cast<const uint32_t *>(q.sign + off));
+                                    const float2 sg = tc05::unpack2<BF16>(*reinterpret_cast<const uint32_t *>(q.sign + off));
                                     v0 = sg.x > 0.0f ? v0 : 0.2f * v0;
                                     v1 = sg.y > 0.0f ? v1 : 0.2f * v1;
                                 }
                                 s1[0] += v0;
                                 s1[1] += v1;
                                 if (q.mod_u) {
-                                    const float2 u = load_pair<true, true>(q.mod_u + off, plane);
+                                    const float2 u = load_pair<X3, BF16>(q.mod_u + off, plane);
                                     s2[0] = fmaf(v0, u.x, s2[0]);
                                     s2[1] = fmaf(v1, u.y, s2[1]);
                                     v0 *= sScale[ch];
@@ -541,7 +549,7 @@ conv_bwd_kernel(const BwdParams q)
                                 if (q.dx) {
                                     if (ch < kInCh) *reinterpret_cast<float2 *>(q.dx + ((size_t)y * p.W + x) * kInCh + ch) = make_float2(v0, v1);
                                 } else {
-                                    store_split2<true, true>(p.out + off, plane, v0, v1);
+                                    store_split2<X3, BF16>(p.out + off, plane, v0, v1);
                                 }
                             }
                         }
@@ -578,14 +586,20 @@ conv_bwd_kernel(const BwdParams q)
 // over CTAs.  Both operands are MN-major straight from the planes: one 8-channel chunk of an item is 64 pixels 16 B apart
 // (K-adjacent core matrices +128 B, MN-adjacent chunks +1 KB); the tap's dx is a 16 B start shift of the input copy, its
 // dy another input row.  fp32 accumulators [128 x cin] stay in two warpgroups' registers for the whole reduction and
-// are added to the zeroed gradient with red.add.  Warp 8 issues the bulk copies into a 2-stage ring.
+// are added to the zeroed gradient with red.add.  Warp 8 issues the bulk copies into a ring of stages: two of 96 KB for
+// bf16 x3 (plane pairs), four of 48 KB for one pass (single planes), whose one product per stage hides less of a copy.
 constexpr int kWgSeg = 64;
 constexpr uint32_t kWgChunk = kWgSeg * 16;               // 1 KB
-constexpr uint32_t kWgGBytes = 2 * 16 * kWgChunk;        // gradient: 2 planes x 128 output channels
-constexpr uint32_t kWgXBytes = 2 * 32 * kWgChunk;        // input: 2 planes x up to 256 channels
-constexpr uint32_t kWgStage = kWgGBytes + kWgXBytes;     // 96 KB
-constexpr uint32_t kWgSmem = 2 * kWgStage + 64;
 constexpr int kWgThreads = 288;
+template <bool X3> struct WgRing {
+    static constexpr uint32_t P = X3 ? 2 : 1;
+    static constexpr uint32_t GBytes = P * 16 * kWgChunk;    // gradient: P planes x 128 output channels
+    static constexpr uint32_t XBytes = P * 32 * kWgChunk;    // input: P planes x up to 256 channels
+    static constexpr uint32_t Stage = GBytes + XBytes;       // 96 KB (x3) or 48 KB
+    static constexpr int LogStages = X3 ? 1 : 2;
+    static constexpr int Stages = 1 << LogStages;
+    static constexpr uint32_t Smem = Stages * Stage + 16 * Stages;
+};
 
 struct WgradParams {
     const uint8_t *g, *in;      // gradient planes (256 channels), input record planes (in_chunks chunks)
@@ -593,12 +607,14 @@ struct WgradParams {
     int in_chunks, taps, H, Hp, Wp, segs, nsplit;
 };
 
-template <int NQ>                                        // 64-channel column blocks of the input: 1 (conv1) or 4
+template <int NQ, bool X3, bool BF16>                    // NQ: 64-channel column blocks of the input: 1 (conv1) or 4
 __global__ void __launch_bounds__(kWgThreads, 1)
 conv_wgrad_kernel(const WgradParams p)
 {
+    using R = WgRing<X3>;
+    constexpr int S = R::Stages, LS = R::LogStages;
     extern __shared__ __align__(1024) uint8_t smem[];
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + 2 * kWgStage);      // full[2], empty[2]
+    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + S * R::Stage);      // full[S], empty[S]
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int job = blockIdx.x / p.nsplit, split = blockIdx.x % p.nsplit;
     const int tap = job >> 1, n0 = (job & 1) * 128;
@@ -606,17 +622,17 @@ conv_wgrad_kernel(const WgradParams p)
     const long long n_items = (long long)p.H * p.segs;
     const long long my_items = split < n_items ? (n_items - split + p.nsplit - 1) / p.nsplit : 0;
     if (tid == 0) {
-        for (int s = 0; s < 2; s++) { tc05::mbar_init(&bars[s], 1); tc05::mbar_init(&bars[2 + s], 2); }
+        for (int s = 0; s < S; s++) { tc05::mbar_init(&bars[s], 1); tc05::mbar_init(&bars[S + s], 2); }
         tc05::fence_mbar_init();
     }
     __syncthreads();
     if (my_items == 0) return;
     if (warp == 8) {
         const size_t gplane = plane_bytes(p.Hp, kCh / 8, p.Wp), xplane = plane_bytes(p.Hp, p.in_chunks, p.Wp);
-        const int n_copies = 32 + 2 * p.in_chunks;
+        const int n_gcopies = (int)R::P * 16, n_copies = n_gcopies + (int)R::P * p.in_chunks;
         for (long long n = 0; n < my_items; n++) {
-            const int s = (int)(n & 1);
-            if (n >= 2) tc05::mbar_wait_backoff(&bars[2 + s], (uint32_t)(((n >> 1) - 1) & 1), 64);
+            const int s = (int)(n & (S - 1));
+            if (n >= S) tc05::mbar_wait_backoff(&bars[S + s], (uint32_t)(((n >> LS) - 1) & 1), 64);
             const long long item = split + n * p.nsplit;
             const int y = (int)(item / p.segs), x0 = (int)(item % p.segs) * kWgSeg;
             if (lane == 0) tc05::mbar_arrive_expect_tx(&bars[s], (uint32_t)n_copies * kWgChunk);
@@ -624,16 +640,16 @@ conv_wgrad_kernel(const WgradParams p)
             for (int i = lane; i < n_copies; i += 32) {
                 const uint8_t *src;
                 uint32_t dst;
-                if (i < 32) {
+                if (i < n_gcopies) {
                     const int pl = i >> 4, c = i & 15;
                     src = p.g + pl * gplane + ((((size_t)(y + 1) * (kCh / 8)) + (n0 >> 3) + c) * p.Wp + x0 + 1) * 16;
                     dst = (uint32_t)(pl * 16 + c) * kWgChunk;
                 } else {
-                    const int pl = (i - 32) / p.in_chunks, c = (i - 32) % p.in_chunks;
+                    const int pl = (i - n_gcopies) / p.in_chunks, c = (i - n_gcopies) % p.in_chunks;
                     src = p.in + pl * xplane + ((((size_t)(y + dy) * p.in_chunks) + c) * p.Wp + x0 + dx) * 16;
-                    dst = kWgGBytes + (uint32_t)(pl * 32 + c) * kWgChunk;
+                    dst = R::GBytes + (uint32_t)(pl * 32 + c) * kWgChunk;
                 }
-                tc05::bulk_g2s(smem + s * kWgStage + dst, src, kWgChunk, &bars[s]);
+                tc05::bulk_g2s(smem + s * R::Stage + dst, src, kWgChunk, &bars[s]);
             }
         }
         return;
@@ -643,19 +659,19 @@ conv_wgrad_kernel(const WgradParams p)
 #pragma unroll
     for (int i = 0; i < NQ * 32; i++) (&acc[0][0])[i] = 0.0f;
     for (long long n = 0; n < my_items; n++) {
-        const int s = (int)(n & 1);
-        tc05::mbar_wait(&bars[s], (uint32_t)((n >> 1) & 1));
-        const uint32_t sG = tc05::smem_u32(smem + s * kWgStage), sX = sG + kWgGBytes;
+        const int s = (int)(n & (S - 1));
+        tc05::mbar_wait(&bars[s], (uint32_t)((n >> LS) & 1));
+        const uint32_t sG = tc05::smem_u32(smem + s * R::Stage), sX = sG + R::GBytes;
         tc05::wgmma_fence();
 #pragma unroll
-        for (int pr = 0; pr < 3; pr++) {                    // g_hi in_hi, g_lo in_hi, g_hi in_lo
+        for (int pr = 0; pr < (X3 ? 3 : 1); pr++) {         // x3: g_hi in_hi, g_lo in_hi, g_hi in_lo
             const uint32_t ga = pr == 1 ? 1u : 0u, xb = pr == 2 ? 1u : 0u;
 #pragma unroll 1
             for (int kk = 0; kk < kWgSeg / 16; kk++) {
                 const uint64_t da = tc05::make_smem_desc(sG + (ga * 16 + wg * 8) * kWgChunk + kk * 256, 128, kWgChunk);
 #pragma unroll
                 for (int q = 0; q < NQ; q++)
-                    tc05::wgmma_m64n64k16<true, 1, 1>(acc[q], da, tc05::make_smem_desc(sX + (xb * 32 + 8 * q) * kWgChunk + kk * 256, 128, kWgChunk), 1u);
+                    tc05::wgmma_m64n64k16<BF16, 1, 1>(acc[q], da, tc05::make_smem_desc(sX + (xb * 32 + 8 * q) * kWgChunk + kk * 256, 128, kWgChunk), 1u);
             }
         }
         tc05::wgmma_commit();
@@ -663,7 +679,7 @@ conv_wgrad_kernel(const WgradParams p)
 #pragma unroll
         for (int q = 0; q < NQ; q++) tc05::wgmma_fence_acc(acc[q]);
         tc05::named_sync(1 + wg, 128);
-        if (t == 0) tc05::mbar_arrive(&bars[2 + s]);
+        if (t == 0) tc05::mbar_arrive(&bars[S + s]);
     }
     const int cin = p.in_chunks * 8;
 #pragma unroll
@@ -741,11 +757,12 @@ static PackLayout pack_layout(int planes) {
     l.total = (o + 255) / 256 * 256;
     return l;
 }
-// data-gradient pack: the 7 transposed layers, 256 input channels each (conv1^T: 256 -> 64, padded to 256), bf16 x3
-static PackLayout bwd_pack_layout() {
+// data-gradient pack: the 7 transposed layers, 256 input channels each (conv1^T: 256 -> 64, padded to 256), in the
+// training path's planes (2: bf16 x3, 1: one pass)
+static PackLayout bwd_pack_layout(int planes) {
     PackLayout l{};
     size_t o = 0;
-    for (int i = 0; i < 7; i++) { l.w[i] = o; o += (size_t)(kCh / 32) * kTaps[i] * 2 * kWStage; }
+    for (int i = 0; i < 7; i++) { l.w[i] = o; o += (size_t)(kCh / 32) * kTaps[i] * planes * kWStage; }
     l.f32 = o;
     l.total = o;
     return l;
@@ -770,15 +787,16 @@ static WsLayout ws_layout(int H, int W, int planes, int &Hp, int &Wp) {
     return l;
 }
 
-// Training record of one view: bf16 plane pairs with zero borders (each u directly before the y it modulates into:
-// conv_kernel<true, bf16> finds u at out - one pair), then rgb [3][H][W] fp32.
+// Training record of one view: `planes` 16-bit planes per activation (bf16 pairs for x3, one plane in the forward's type for
+// one pass) with zero borders, each u directly before the y it modulates into (conv_kernel<., ., true> finds u at out -
+// planes), then rgb [3][H][W] fp32.
 struct RecLayout { size_t x, y1, t1, u2, y2, t2, u3, y3, t3, y4, rgb, total; };
-static RecLayout rec_layout(int H, int W, int &Hp, int &Wp) {
+static RecLayout rec_layout(int H, int W, int planes, int &Hp, int &Wp) {
     padded_dims(H, W, Hp, Wp);
     RecLayout l{};
     size_t o = 0;
-    l.x = o; o += (plane_bytes(Hp, kInCh / 8, Wp) * 2 + 255) / 256 * 256;
-    const size_t big = plane_bytes(Hp, kCh / 8, Wp) * 2;     // a multiple of 512 B
+    l.x = o; o += (plane_bytes(Hp, kInCh / 8, Wp) * planes + 255) / 256 * 256;
+    const size_t big = plane_bytes(Hp, kCh / 8, Wp) * planes;     // a multiple of 512 B
     size_t *pairs[9] = {&l.y1, &l.t1, &l.u2, &l.y2, &l.t2, &l.u3, &l.y3, &l.t3, &l.y4};
     for (int i = 0; i < 9; i++) { *pairs[i] = o; o += big; }
     l.rgb = o; o += ((size_t)3 * H * W * 4 + 255) / 256 * 256;
@@ -786,17 +804,17 @@ static RecLayout rec_layout(int H, int W, int &Hp, int &Wp) {
     return l;
 }
 
-// Backward workspace: three gradient plane pairs in rotation
-static size_t bwd_ws_bytes(int H, int W, int &Hp, int &Wp) {
+// Backward workspace: three gradient tensors of `planes` planes in rotation
+static size_t bwd_ws_bytes(int H, int W, int planes, int &Hp, int &Wp) {
     padded_dims(H, W, Hp, Wp);
-    return 3 * plane_bytes(Hp, kCh / 8, Wp) * 2;
+    return 3 * plane_bytes(Hp, kCh / 8, Wp) * planes;
 }
 
 // one forward layer table entry: byte offsets into the activation buffer (NONE = absent)
 struct FwdLayer { size_t in, res, out; int in_chunks, epi; const float *bias, *mw, *mb; };
 constexpr size_t NONE = (size_t)-1;
 
-template <bool X3, bool BF16>
+template <bool X3, bool BF16, bool REC>
 static int launch_forward_layers(const FwdLayer (&layers)[7], uint8_t *buf, const uint8_t *pack, const PackLayout &pl,
                                  LayerParams base, float *d_rgb, float *d_rgb_raw, cudaStream_t st)
 {
@@ -814,8 +832,8 @@ static int launch_forward_layers(const FwdLayer (&layers)[7], uint8_t *buf, cons
         p.in_chunks = l.in_chunks; p.taps = kTaps[i]; p.epi = l.epi;
         if (l.epi == EPI_RES_BIAS_LRELU_RGB) { p.w4 = f + 5 * kCh; p.b4 = f + 8 * kCh; p.rgb = d_rgb; p.rgb_raw = d_rgb_raw; }
         const uint32_t smem = smem_map(p.taps, X3 ? 2 : 1).total;
-        SDB_CUDA(cudaFuncSetAttribute(conv_kernel<X3, BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        conv_kernel<X3, BF16><<<grid, kThreads, smem, st>>>(p);
+        SDB_CUDA(cudaFuncSetAttribute(conv_kernel<X3, BF16, REC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        conv_kernel<X3, BF16, REC><<<grid, kThreads, smem, st>>>(p);
         SDB_CHECK_LAUNCH();
     }
     return SDB_OK;
@@ -828,26 +846,35 @@ static LayerParams frame_params(int H, int W, int Hp, int Wp, int planes) {
     return base;
 }
 
+// pack precisions: 0 = fp16 x1, 1 = bf16 x3, 2 = fp16 x3, 3 = bf16 x1 (the one-pass bf16 training path only)
+static int pack_planes(int precision) { return precision == 0 || precision == 3 ? 1 : 2; }
+
 }  // namespace cnn
+
+extern "C" int64_t sdb_cnn_pack_bytes_ex(int32_t precision) {
+    if (precision < 0 || precision > 3) return 0;
+    return (int64_t)cnn::pack_layout(cnn::pack_planes(precision)).total;
+}
 
 extern "C" int64_t sdb_cnn_pack_bytes(int32_t precision) {
     if (precision < 0 || precision > 2) return 0;
-    return (int64_t)cnn::pack_layout(precision == 0 ? 1 : 2).total;
+    return sdb_cnn_pack_bytes_ex(precision);
 }
 
 // Device fp32 tensors with the reference's state-dict shapes (denoiser.*): conv1 [256,64,1,1] + [256]; conv2a / conv3a
 // [256,256,3,3] + [256]; conv2b / conv3b [256,256,3,3] (no bias); conv4a / conv4b [256,256,1,1] + [256]; conv4 [3,256,1,1] + [3].
-extern "C" int sdb_cnn_pack(const float *d_w1, const float *d_b1, const float *d_w2a, const float *d_b2a, const float *d_w2b,
-                            const float *d_w3a, const float *d_b3a, const float *d_w3b, const float *d_w4a, const float *d_b4a,
-                            const float *d_w4b, const float *d_b4b, const float *d_w4, const float *d_b4, int32_t precision,
-                            void *d_pack, void *stream)
+extern "C" int sdb_cnn_pack_ex(const float *d_w1, const float *d_b1, const float *d_w2a, const float *d_b2a, const float *d_w2b,
+                               const float *d_w3a, const float *d_b3a, const float *d_w3b, const float *d_w4a, const float *d_b4a,
+                               const float *d_w4b, const float *d_b4b, const float *d_w4, const float *d_b4, int32_t precision,
+                               void *d_pack, void *stream)
 {
     using namespace cnn;
     if (!d_w1 || !d_b1 || !d_w2a || !d_b2a || !d_w2b || !d_w3a || !d_b3a || !d_w3b || !d_w4a || !d_b4a || !d_w4b || !d_b4b || !d_w4 ||
         !d_b4 || !d_pack)
         return SDB_EINVAL;
-    if (precision < 0 || precision > 2) return SDB_EUNSUPPORTED;
-    const int planes = precision == 0 ? 1 : 2;
+    if (precision < 0 || precision > 3) return SDB_EUNSUPPORTED;
+    const int planes = pack_planes(precision);
+    const bool bf16 = precision == 1 || precision == 3;
     const PackLayout l = pack_layout(planes);
     cudaStream_t st = (cudaStream_t)stream;
     const float *ws[7] = {d_w1, d_w2a, d_w2b, d_w3a, d_w3b, d_w4a, d_w4b};
@@ -856,7 +883,7 @@ extern "C" int sdb_cnn_pack(const float *d_w1, const float *d_b1, const float *d
         const long long n = (long long)kCh * cin[i] * kTaps[i];
         const unsigned blocks = (unsigned)((n + 255) / 256);
         uint8_t *dst = (uint8_t *)d_pack + l.w[i];
-        if (precision == 1) pack_weight_kernel<true, false><<<blocks, 256, 0, st>>>(ws[i], dst, cin[i], kTaps[i], planes, kCh);
+        if (bf16) pack_weight_kernel<true, false><<<blocks, 256, 0, st>>>(ws[i], dst, cin[i], kTaps[i], planes, kCh);
         else pack_weight_kernel<false, false><<<blocks, 256, 0, st>>>(ws[i], dst, cin[i], kTaps[i], planes, kCh);
         SDB_CHECK_LAUNCH();
     }
@@ -866,6 +893,19 @@ extern "C" int sdb_cnn_pack(const float *d_w1, const float *d_b1, const float *d
     SDB_CUDA(cudaMemcpyAsync(f + 5 * kCh, d_w4, 3 * kCh * 4, cudaMemcpyDeviceToDevice, st));
     SDB_CUDA(cudaMemcpyAsync(f + 8 * kCh, d_b4, 3 * 4, cudaMemcpyDeviceToDevice, st));
     return SDB_OK;
+}
+
+extern "C" int sdb_cnn_pack(const float *d_w1, const float *d_b1, const float *d_w2a, const float *d_b2a, const float *d_w2b,
+                            const float *d_w3a, const float *d_b3a, const float *d_w3b, const float *d_w4a, const float *d_b4a,
+                            const float *d_w4b, const float *d_b4b, const float *d_w4, const float *d_b4, int32_t precision,
+                            void *d_pack, void *stream)
+{
+    if (!d_w1 || !d_b1 || !d_w2a || !d_b2a || !d_w2b || !d_w3a || !d_b3a || !d_w3b || !d_w4a || !d_b4a || !d_w4b || !d_b4b || !d_w4 ||
+        !d_b4 || !d_pack)
+        return SDB_EINVAL;
+    if (precision < 0 || precision > 2) return SDB_EUNSUPPORTED;
+    return sdb_cnn_pack_ex(d_w1, d_b1, d_w2a, d_b2a, d_w2b, d_w3a, d_b3a, d_w3b, d_w4a, d_b4a, d_w4b, d_b4b, d_w4, d_b4, precision,
+                           d_pack, stream);
 }
 
 extern "C" int64_t sdb_cnn_workspace_bytes(int32_t H, int32_t W, int32_t precision) {
@@ -909,46 +949,58 @@ extern "C" int sdb_cnn_forward(const float *d_net_out, int32_t H, int32_t W, con
         {wl.t, wl.y, NONE, kCh / 8, EPI_RES_BIAS_LRELU_RGB, f + 4 * kCh, nullptr, nullptr},                   // conv4b, conv4, tanh
     };
     const LayerParams base = frame_params(H, W, Hp, Wp, planes);
-    if (planes == 2) return launch_forward_layers<true, false>(layers, ws, pack, pl, base, d_rgb, d_rgb_raw, st);
-    return launch_forward_layers<false, false>(layers, ws, pack, pl, base, d_rgb, d_rgb_raw, st);
+    if (planes == 2) return launch_forward_layers<true, false, false>(layers, ws, pack, pl, base, d_rgb, d_rgb_raw, st);
+    return launch_forward_layers<false, false, false>(layers, ws, pack, pl, base, d_rgb, d_rgb_raw, st);
 }
 
 // ---------------------------------------------- training (include/sdb200.h, f1 under autograd) ----------------------------------------------
-extern "C" int64_t sdb_cnn_train_record_bytes(int32_t H, int32_t W) {
-    if (H <= 0 || W <= 0) return 0;
+// Training precisions: 0 = fp16 x1, 1 = bf16 x3, 3 = bf16 x1; pack, record, backward pack and workspace of one training pass
+// all come from the same precision.  The entries without _ex are precision 1.
+static bool train_precision_ok(int32_t precision) { return precision == 0 || precision == 1 || precision == 3; }
+
+extern "C" int64_t sdb_cnn_train_record_bytes_ex(int32_t H, int32_t W, int32_t precision) {
+    if (H <= 0 || W <= 0 || !train_precision_ok(precision)) return 0;
     int Hp, Wp;
-    return (int64_t)cnn::rec_layout(H, W, Hp, Wp).total;
+    return (int64_t)cnn::rec_layout(H, W, cnn::pack_planes(precision), Hp, Wp).total;
 }
 
-// Diagnostics: Hp, Wp, then the byte offsets of the record's x, y1, t1, u2, y2, t2, u3, y3, t3, y4 plane pairs and of rgb,
-// then the record size -- 14 int64 in all.  A pair is [hi, lo] bf16 planes of [Hp][channels / 8][Wp][8]; pixel (y, x) sits
-// at row y + 1, column x + 1.
-extern "C" int sdb_cnn_debug_record_layout(int32_t H, int32_t W, int64_t *out)
+extern "C" int64_t sdb_cnn_train_record_bytes(int32_t H, int32_t W) { return sdb_cnn_train_record_bytes_ex(H, W, 1); }
+
+// Diagnostics: Hp, Wp, then the byte offsets of the record's x, y1, t1, u2, y2, t2, u3, y3, t3, y4 planes and of rgb, then
+// the record size -- 14 int64 in all.  An activation is `planes` 16-bit planes of [Hp][channels / 8][Wp][8] (bf16 [hi, lo]
+// at precision 1, one plane of the forward's type at 0 and 3); pixel (y, x) sits at row y + 1, column x + 1.
+extern "C" int sdb_cnn_debug_record_layout_ex(int32_t H, int32_t W, int32_t precision, int64_t *out)
 {
     if (!out || H <= 0 || W <= 0) return SDB_EINVAL;
+    if (!train_precision_ok(precision)) return SDB_EUNSUPPORTED;
     int Hp, Wp;
-    const cnn::RecLayout r = cnn::rec_layout(H, W, Hp, Wp);
+    const cnn::RecLayout r = cnn::rec_layout(H, W, cnn::pack_planes(precision), Hp, Wp);
     const size_t v[14] = {(size_t)Hp, (size_t)Wp, r.x, r.y1, r.t1, r.u2, r.y2, r.t2, r.u3, r.y3, r.t3, r.y4, r.rgb, r.total};
     for (int i = 0; i < 14; i++) out[i] = (int64_t)v[i];
     return SDB_OK;
 }
 
-extern "C" int sdb_cnn_train_forward(const float *d_net_out, int32_t H, int32_t W, const void *d_pack, const float *d_mod,
-                                     float *d_rgb, float *d_rgb_raw, void *d_record, void *stream)
+extern "C" int sdb_cnn_debug_record_layout(int32_t H, int32_t W, int64_t *out) { return sdb_cnn_debug_record_layout_ex(H, W, 1, out); }
+
+extern "C" int sdb_cnn_train_forward_ex(const float *d_net_out, int32_t H, int32_t W, const void *d_pack, const float *d_mod,
+                                        int32_t precision, float *d_rgb, float *d_rgb_raw, void *d_record, void *stream)
 {
     using namespace cnn;
     if (!d_net_out || !d_pack || !d_mod || !d_rgb || !d_record || H <= 0 || W <= 0) return SDB_EINVAL;
+    if (!train_precision_ok(precision)) return SDB_EUNSUPPORTED;
+    const int planes = pack_planes(precision);
     cudaStream_t st = (cudaStream_t)stream;
     int Hp, Wp;
-    const RecLayout r = rec_layout(H, W, Hp, Wp);
-    const PackLayout pl = pack_layout(2);
+    const RecLayout r = rec_layout(H, W, planes, Hp, Wp);
+    const PackLayout pl = pack_layout(planes);
     uint8_t *rec = (uint8_t *)d_record;
     const uint8_t *pack = (const uint8_t *)d_pack;
     const float *f = reinterpret_cast<const float *>(pack + pl.f32);
     SDB_CUDA(cudaMemsetAsync(rec, 0, r.rgb, st));                     // the zero borders (and the area past the frame)
     {
         const long long n = (long long)H * W * (kInCh / 8);
-        pack_input_kernel<true><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_net_out, rec + r.x, H, W, Hp, Wp, 2);
+        if (precision == 0) pack_input_kernel<false><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_net_out, rec + r.x, H, W, Hp, Wp, planes);
+        else pack_input_kernel<true><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_net_out, rec + r.x, H, W, Hp, Wp, planes);
         SDB_CHECK_LAUNCH();
     }
     const FwdLayer layers[7] = {
@@ -960,53 +1012,144 @@ extern "C" int sdb_cnn_train_forward(const float *d_net_out, int32_t H, int32_t 
         {r.y3, NONE, r.t3, kCh / 8, EPI_BIAS_LRELU, f + 3 * kCh, nullptr, nullptr},                           // conv4a
         {r.t3, r.y3, r.y4, kCh / 8, EPI_RES_BIAS_LRELU_RGB, f + 4 * kCh, nullptr, nullptr},                   // conv4b (y4), conv4, tanh
     };
-    const int rc = launch_forward_layers<true, true>(layers, rec, pack, pl, frame_params(H, W, Hp, Wp, 2), d_rgb, d_rgb_raw, st);
+    const LayerParams base = frame_params(H, W, Hp, Wp, planes);
+    int rc;
+    if (precision == 1) rc = launch_forward_layers<true, true, true>(layers, rec, pack, pl, base, d_rgb, d_rgb_raw, st);
+    else if (precision == 3) rc = launch_forward_layers<false, true, true>(layers, rec, pack, pl, base, d_rgb, d_rgb_raw, st);
+    else rc = launch_forward_layers<false, false, true>(layers, rec, pack, pl, base, d_rgb, d_rgb_raw, st);
     if (rc != SDB_OK) return rc;
     SDB_CUDA(cudaMemcpyAsync(rec + r.rgb, d_rgb, (size_t)3 * H * W * 4, cudaMemcpyDeviceToDevice, st));
     return SDB_OK;
 }
 
-extern "C" int64_t sdb_cnn_backward_pack_bytes(void) { return (int64_t)cnn::bwd_pack_layout().total; }
+extern "C" int sdb_cnn_train_forward(const float *d_net_out, int32_t H, int32_t W, const void *d_pack, const float *d_mod,
+                                     float *d_rgb, float *d_rgb_raw, void *d_record, void *stream)
+{
+    return sdb_cnn_train_forward_ex(d_net_out, H, W, d_pack, d_mod, 1, d_rgb, d_rgb_raw, d_record, stream);
+}
 
-extern "C" int sdb_cnn_pack_backward(const float *d_w1, const float *d_w2a, const float *d_w2b, const float *d_w3a,
-                                     const float *d_w3b, const float *d_w4a, const float *d_w4b, void *d_pack, void *stream)
+extern "C" int64_t sdb_cnn_backward_pack_bytes_ex(int32_t precision) {
+    if (!train_precision_ok(precision)) return 0;
+    return (int64_t)cnn::bwd_pack_layout(cnn::pack_planes(precision)).total;
+}
+
+extern "C" int64_t sdb_cnn_backward_pack_bytes(void) { return sdb_cnn_backward_pack_bytes_ex(1); }
+
+extern "C" int sdb_cnn_pack_backward_ex(const float *d_w1, const float *d_w2a, const float *d_w2b, const float *d_w3a,
+                                        const float *d_w3b, const float *d_w4a, const float *d_w4b, int32_t precision, void *d_pack,
+                                        void *stream)
 {
     using namespace cnn;
     if (!d_w1 || !d_w2a || !d_w2b || !d_w3a || !d_w3b || !d_w4a || !d_w4b || !d_pack) return SDB_EINVAL;
-    const PackLayout l = bwd_pack_layout();
+    if (!train_precision_ok(precision)) return SDB_EUNSUPPORTED;
+    const int planes = pack_planes(precision);
+    const PackLayout l = bwd_pack_layout(planes);
     cudaStream_t st = (cudaStream_t)stream;
     const float *ws[7] = {d_w1, d_w2a, d_w2b, d_w3a, d_w3b, d_w4a, d_w4b};
     for (int i = 0; i < 7; i++) {
         const long long n = (long long)kCh * kCh * kTaps[i];
-        pack_weight_kernel<true, true><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ws[i], (uint8_t *)d_pack + l.w[i], kCh, kTaps[i], 2,
-                                                                                     i == 0 ? kInCh : kCh);
+        const unsigned blocks = (unsigned)((n + 255) / 256);
+        uint8_t *dst = (uint8_t *)d_pack + l.w[i];
+        if (precision == 0) pack_weight_kernel<false, true><<<blocks, 256, 0, st>>>(ws[i], dst, kCh, kTaps[i], planes, i == 0 ? kInCh : kCh);
+        else pack_weight_kernel<true, true><<<blocks, 256, 0, st>>>(ws[i], dst, kCh, kTaps[i], planes, i == 0 ? kInCh : kCh);
         SDB_CHECK_LAUNCH();
     }
     return SDB_OK;
 }
 
-extern "C" int64_t sdb_cnn_backward_workspace_bytes(int32_t H, int32_t W) {
-    if (H <= 0 || W <= 0) return 0;
-    int Hp, Wp;
-    return (int64_t)cnn::bwd_ws_bytes(H, W, Hp, Wp);
+extern "C" int sdb_cnn_pack_backward(const float *d_w1, const float *d_w2a, const float *d_w2b, const float *d_w3a,
+                                     const float *d_w3b, const float *d_w4a, const float *d_w4b, void *d_pack, void *stream)
+{
+    return sdb_cnn_pack_backward_ex(d_w1, d_w2a, d_w2b, d_w3a, d_w3b, d_w4a, d_w4b, 1, d_pack, stream);
 }
 
-extern "C" int sdb_cnn_backward(int32_t H, int32_t W, const void *d_record, const float *d_grad_rgb, const float *d_grad_rgb_raw,
-                                const void *d_bwd_pack, const void *d_pack, const float *d_mod, const sdb_cnn_grads *g,
-                                void *d_workspace, void *stream)
+extern "C" int64_t sdb_cnn_backward_workspace_bytes_ex(int32_t H, int32_t W, int32_t precision) {
+    if (H <= 0 || W <= 0 || !train_precision_ok(precision)) return 0;
+    int Hp, Wp;
+    return (int64_t)cnn::bwd_ws_bytes(H, W, cnn::pack_planes(precision), Hp, Wp);
+}
+
+extern "C" int64_t sdb_cnn_backward_workspace_bytes(int32_t H, int32_t W) { return sdb_cnn_backward_workspace_bytes_ex(H, W, 1); }
+
+namespace cnn {
+
+struct BwdStep { int layer; int gin, gres, gout; size_t sign, u, x; const float *mw; float *s1, *s2, *dw; int x_chunks; };
+
+// the data and weight gradient steps of the conv layers, from the last to the first (see sdb_cnn_backward_ex)
+template <bool X3, bool BF16>
+static int launch_backward_layers(const BwdStep (&steps)[7], const uint8_t *rec, const uint8_t *bpack, const PackLayout &bl,
+                                  uint8_t *const (&G)[3], const LayerParams &base, float *d_grad_net_out, cudaStream_t st)
+{
+    using R = WgRing<X3>;
+    const int n_tiles = base.tiles_x * base.tiles_y, sms = sdb_num_sms();
+    const int grid = n_tiles < sms ? n_tiles : sms;
+    for (int i = 0; i < 7; i++) {
+        const BwdStep &s = steps[i];
+        if (s.layer > 0 || d_grad_net_out) {
+            BwdParams q{};
+            q.l = base;
+            q.l.in = G[s.gin];
+            q.l.res = s.gres < 0 ? nullptr : G[s.gres];
+            q.l.out = s.gout < 0 ? nullptr : G[s.gout];
+            q.l.wpack = bpack + bl.w[s.layer];
+            q.l.mod_w = s.mw;
+            q.l.in_chunks = kCh / 8;
+            q.l.taps = kTaps[s.layer];
+            q.sign = s.sign == NONE ? nullptr : rec + s.sign;
+            q.mod_u = s.u == NONE ? nullptr : rec + s.u;
+            q.sum1 = s.s1; q.sum2 = s.s2;
+            q.dx = s.layer == 0 ? d_grad_net_out : nullptr;
+            const uint32_t smem = smem_map(q.l.taps, X3 ? 2 : 1).total;
+            SDB_CUDA(cudaFuncSetAttribute(conv_bwd_kernel<X3, BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            conv_bwd_kernel<X3, BF16><<<grid, kThreads, smem, st>>>(q);
+            SDB_CHECK_LAUNCH();
+        }
+        if (s.dw) {
+            WgradParams w{};
+            w.g = G[s.gin];
+            w.in = rec + s.x;
+            w.dw = s.dw;
+            w.in_chunks = s.x_chunks;
+            w.taps = kTaps[s.layer];
+            w.H = base.H; w.Hp = base.Hp; w.Wp = base.Wp; w.segs = (base.Wp - 2) / kWgSeg;
+            const int jobs = 2 * w.taps;
+            const long long n_items = (long long)base.H * w.segs;
+            long long ns = (2LL * sms + jobs - 1) / jobs;
+            if (ns > n_items) ns = n_items;
+            w.nsplit = (int)ns;
+            if (w.in_chunks == kInCh / 8) {
+                SDB_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel<1, X3, BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)R::Smem));
+                conv_wgrad_kernel<1, X3, BF16><<<(unsigned)(jobs * w.nsplit), kWgThreads, R::Smem, st>>>(w);
+            } else {
+                SDB_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel<4, X3, BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)R::Smem));
+                conv_wgrad_kernel<4, X3, BF16><<<(unsigned)(jobs * w.nsplit), kWgThreads, R::Smem, st>>>(w);
+            }
+            SDB_CHECK_LAUNCH();
+        }
+    }
+    return SDB_OK;
+}
+
+}  // namespace cnn
+
+extern "C" int sdb_cnn_backward_ex(int32_t H, int32_t W, int32_t precision, const void *d_record, const float *d_grad_rgb,
+                                   const float *d_grad_rgb_raw, const void *d_bwd_pack, const void *d_pack, const float *d_mod,
+                                   const sdb_cnn_grads *g, void *d_workspace, void *stream)
 {
     using namespace cnn;
     if (!d_record || (!d_grad_rgb && !d_grad_rgb_raw) || !d_bwd_pack || !d_pack || !d_mod || !g || !d_workspace || H <= 0 || W <= 0)
         return SDB_EINVAL;
+    if (!train_precision_ok(precision)) return SDB_EUNSUPPORTED;
+    const int planes = pack_planes(precision);
     cudaStream_t st = (cudaStream_t)stream;
     int Hp, Wp;
-    const RecLayout r = rec_layout(H, W, Hp, Wp);
-    const size_t pair = plane_bytes(Hp, kCh / 8, Wp) * 2;
-    const PackLayout bl = bwd_pack_layout(), pl = pack_layout(2);
+    const RecLayout r = rec_layout(H, W, planes, Hp, Wp);
+    const size_t gbytes = plane_bytes(Hp, kCh / 8, Wp) * planes;
+    const PackLayout bl = bwd_pack_layout(planes), pl = pack_layout(planes);
     const uint8_t *rec = (const uint8_t *)d_record, *bpack = (const uint8_t *)d_bwd_pack;
     const float *f = reinterpret_cast<const float *>((const uint8_t *)d_pack + pl.f32);
-    uint8_t *G[3] = {(uint8_t *)d_workspace, (uint8_t *)d_workspace + pair, (uint8_t *)d_workspace + 2 * pair};
-    SDB_CUDA(cudaMemsetAsync(d_workspace, 0, 3 * pair, st));
+    uint8_t *const G[3] = {(uint8_t *)d_workspace, (uint8_t *)d_workspace + gbytes, (uint8_t *)d_workspace + 2 * gbytes};
+    SDB_CUDA(cudaMemsetAsync(d_workspace, 0, 3 * gbytes, st));
     float *zeroed[16] = {g->d_grad_mod, g->d_grad_w1, g->d_grad_b1, g->d_grad_w2a, g->d_grad_b2a, g->d_grad_w2b, g->d_grad_w3a,
                          g->d_grad_b3a, g->d_grad_w3b, g->d_grad_w4a, g->d_grad_b4a, g->d_grad_w4b, g->d_grad_b4b, g->d_grad_w4, g->d_grad_b4, nullptr};
     const size_t zbytes[15] = {4 * kCh, (size_t)kCh * kInCh, kCh, (size_t)kCh * kCh * 9, kCh, (size_t)kCh * kCh * 9, (size_t)kCh * kCh * 9,
@@ -1023,14 +1166,16 @@ extern "C" int sdb_cnn_backward(int32_t H, int32_t W, const void *d_record, cons
         const long long HW = (long long)H * W;
         long long bx = (HW + 255) / 256;
         if (bx > sdb_num_sms()) bx = sdb_num_sms();                                      // x 32 chunks: 32 blocks of 256 per SM
-        head_bwd_kernel<<<dim3((unsigned)bx, kCh / 8), 256, 0, st>>>(h);
+        const dim3 grid((unsigned)bx, kCh / 8);
+        if (precision == 1) head_bwd_kernel<true, true><<<grid, 256, 0, st>>>(h);
+        else if (precision == 3) head_bwd_kernel<false, true><<<grid, 256, 0, st>>>(h);
+        else head_bwd_kernel<false, false><<<grid, 256, 0, st>>>(h);
         SDB_CHECK_LAUNCH();
     }
     // the conv layers from the last to the first: data gradient, then the layer's weight gradient, which reads the gradient at
     // the layer's output (the input of its data step, G[gin]) and the layer's input from the record (x)
-    struct Step { int layer; int gin, gres, gout; size_t sign, u, x; const float *mw; float *s1, *s2, *dw; int x_chunks; };
     const int N_ = -1;
-    const Step steps[7] = {
+    const BwdStep steps[7] = {
         {6, 0, N_, 1, r.t3, NONE, r.t3, nullptr, g->d_grad_b4a, nullptr, g->d_grad_w4b, kCh / 8},                      // conv4b^T -> g_p4a
         {5, 1, 0, 2, r.y3, r.u3, r.y3, d_mod + 2 * kCh, dm ? dm + 3 * kCh : nullptr, dm ? dm + 2 * kCh : nullptr, g->d_grad_w4a, kCh / 8},   // conv4a^T -> g_u3
         {4, 2, N_, 0, r.t2, NONE, r.t2, nullptr, g->d_grad_b3a, nullptr, g->d_grad_w3b, kCh / 8},                      // conv3b^T -> g_p3a
@@ -1039,52 +1184,15 @@ extern "C" int sdb_cnn_backward(int32_t H, int32_t W, const void *d_record, cons
         {1, 2, 1, 0, r.y1, NONE, r.y1, nullptr, g->d_grad_b1, nullptr, g->d_grad_w2a, kCh / 8},                        // conv2a^T -> g_p1
         {0, 0, N_, N_, NONE, NONE, r.x, nullptr, nullptr, nullptr, g->d_grad_w1, kInCh / 8},                          // conv1^T -> dL/dnet_out
     };
-    const LayerParams base = frame_params(H, W, Hp, Wp, 2);
-    const int n_tiles = base.tiles_x * base.tiles_y, sms = sdb_num_sms();
-    const int grid = n_tiles < sms ? n_tiles : sms;
-    for (int i = 0; i < 7; i++) {
-        const Step &s = steps[i];
-        if (s.layer > 0 || g->d_grad_net_out) {
-            BwdParams q{};
-            q.l = base;
-            q.l.in = G[s.gin];
-            q.l.res = s.gres < 0 ? nullptr : G[s.gres];
-            q.l.out = s.gout < 0 ? nullptr : G[s.gout];
-            q.l.wpack = bpack + bl.w[s.layer];
-            q.l.mod_w = s.mw;
-            q.l.in_chunks = kCh / 8;
-            q.l.taps = kTaps[s.layer];
-            q.sign = s.sign == NONE ? nullptr : rec + s.sign;
-            q.mod_u = s.u == NONE ? nullptr : rec + s.u;
-            q.sum1 = s.s1; q.sum2 = s.s2;
-            q.dx = s.layer == 0 ? g->d_grad_net_out : nullptr;
-            const uint32_t smem = smem_map(q.l.taps, 2).total;
-            SDB_CUDA(cudaFuncSetAttribute(conv_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            conv_bwd_kernel<<<grid, kThreads, smem, st>>>(q);
-            SDB_CHECK_LAUNCH();
-        }
-        if (s.dw) {
-            WgradParams w{};
-            w.g = G[s.gin];
-            w.in = rec + s.x;
-            w.dw = s.dw;
-            w.in_chunks = s.x_chunks;
-            w.taps = kTaps[s.layer];
-            w.H = H; w.Hp = Hp; w.Wp = Wp; w.segs = (Wp - 2) / kWgSeg;
-            const int jobs = 2 * w.taps;
-            const long long n_items = (long long)H * w.segs;
-            long long ns = (2LL * sms + jobs - 1) / jobs;
-            if (ns > n_items) ns = n_items;
-            w.nsplit = (int)ns;
-            if (w.in_chunks == kInCh / 8) {
-                SDB_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kWgSmem));
-                conv_wgrad_kernel<1><<<(unsigned)(jobs * w.nsplit), kWgThreads, kWgSmem, st>>>(w);
-            } else {
-                SDB_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kWgSmem));
-                conv_wgrad_kernel<4><<<(unsigned)(jobs * w.nsplit), kWgThreads, kWgSmem, st>>>(w);
-            }
-            SDB_CHECK_LAUNCH();
-        }
-    }
-    return SDB_OK;
+    const LayerParams base = frame_params(H, W, Hp, Wp, planes);
+    if (precision == 1) return launch_backward_layers<true, true>(steps, rec, bpack, bl, G, base, g->d_grad_net_out, st);
+    if (precision == 3) return launch_backward_layers<false, true>(steps, rec, bpack, bl, G, base, g->d_grad_net_out, st);
+    return launch_backward_layers<false, false>(steps, rec, bpack, bl, G, base, g->d_grad_net_out, st);
+}
+
+extern "C" int sdb_cnn_backward(int32_t H, int32_t W, const void *d_record, const float *d_grad_rgb, const float *d_grad_rgb_raw,
+                                const void *d_bwd_pack, const void *d_pack, const float *d_mod, const sdb_cnn_grads *g,
+                                void *d_workspace, void *stream)
+{
+    return sdb_cnn_backward_ex(H, W, 1, d_record, d_grad_rgb, d_grad_rgb_raw, d_bwd_pack, d_pack, d_mod, g, d_workspace, stream);
 }

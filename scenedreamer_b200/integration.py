@@ -61,6 +61,21 @@ def train_recompute_enabled():
     return os.environ.get('SDB200_TRAIN_RECOMPUTE', '0') not in ('0', 'false', 'False', 'off', '')
 
 
+def cnn_amp_enabled():
+    """SDB200_CNN_AMP=1: a RenderCNN call that needs gradients under torch.autocast trains on the tensor cores in one pass
+    of autocast's dtype (rendercnn.PRECISION_FP16 under fp16 autocast, PRECISION_BF16 under bf16) instead of the
+    reference's composition.  Off by default."""
+    return os.environ.get('SDB200_CNN_AMP', '0') not in ('0', 'false', 'False', 'off', '')
+
+
+def cnn_amp_precision():
+    """Training precision of the RenderCNN under the current autocast, or None when autocast's dtype has no one-pass
+    path.  It follows autocast's dtype, unlike the per-pixel MLP's fp16 under both: bf16 autocast runs without a
+    GradScaler, and there fp16 gradient planes would hold the ~1e-5 gradients of a mean loss as subnormals."""
+    return {torch.float16: rendercnn.PRECISION_FP16, torch.bfloat16: rendercnn.PRECISION_BF16}.get(
+        torch.get_autocast_dtype('cuda'))
+
+
 # ------------------------------------------------------------------------------------------------
 # per-instance state
 # ------------------------------------------------------------------------------------------------
@@ -94,7 +109,7 @@ class _FusedState:
         self.frame = _FrameCache()
         self.stats = {'fused_calls': 0, 'frame_launches': 0, 'tile_hits': 0, 'train_calls': 0, 'reference_calls': 0,
                       'cnn_frame_launches': 0, 'cnn_tile_hits': 0, 'cnn_calls': 0, 'cnn_reference_calls': 0,
-                      'cnn_train_calls': 0, 'train_recompute_calls': 0}
+                      'cnn_train_calls': 0, 'cnn_amp_train_calls': 0, 'train_recompute_calls': 0}
 
     @property
     def lut(self):
@@ -352,22 +367,29 @@ def fused_forward_global(self, net_out, z):
     inference_givenstyle), the CNN runs ONCE on the whole padded frame and every tile gets its window: the receptive
     radius is 4 px, the loop crops pad/2 = 15 px from every tile side (DESIGN.md section 1).  Calls that need gradients
     through the CNN (gen_update) run the recording bf16 x3 forward, whose backward is the library's as well
-    (rendercnn._RenderCNNTrainFn); under autocast they keep the reference's composition."""
+    (rendercnn._RenderCNNTrainFn); under autocast they keep the reference's composition unless SDB200_CNN_AMP=1, which
+    trains them in one pass of autocast's dtype (cnn_amp_precision)."""
     st = _state(self)
     reference = type(self)._sdb200_reference_forward_global
     needs_grad = torch.is_grad_enabled() and (net_out.requires_grad or (z is not None and z.requires_grad) or
                                               any(q.requires_grad for q in self.denoiser.parameters()))
+    amp_train = needs_grad and torch.is_autocast_enabled()
+    amp_precision = cnn_amp_precision() if amp_train and cnn_amp_enabled() else None
     eng = None
     if enabled() and os.environ.get('SDB200_CNN', '1') != '0' and z is not None and net_out.is_cuda and \
             net_out.dim() == 4 and net_out.shape[-1] == 64 and net_out.dtype == torch.float32 and \
-            not (needs_grad and torch.is_autocast_enabled()):
+            (not amp_train or amp_precision is not None):
         eng = st.get_cnn(self)
     if eng is None:
         st.stats['cnn_reference_calls'] += 1
         return reference(self, net_out, z)
     if needs_grad:
         st.stats['cnn_train_calls'] += 1
-        return eng.forward_train(net_out, z, {'denoiser.' + k: v for k, v in self.denoiser.named_parameters()})
+        P = {'denoiser.' + k: v for k, v in self.denoiser.named_parameters()}
+        if amp_train:
+            st.stats['cnn_amp_train_calls'] += 1
+            return eng.forward_train(net_out, z, P, precision=amp_precision)
+        return eng.forward_train(net_out, z, P)
     full = st.frame.out
     if full is not None and net_out.shape[0] == 1 and z.shape[0] == 1:
         base = full['net_out']

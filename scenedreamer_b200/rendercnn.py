@@ -1,5 +1,5 @@
 """Host side of the tensor-core RenderCNN (libsdb200: sdb_cnn_pack / sdb_cnn_forward, and under autograd
-sdb_cnn_train_forward / sdb_cnn_backward).
+sdb_cnn_train_forward_ex / sdb_cnn_backward_ex).
 
 Mirrors Base3DGenerator._forward_global (imaginaire/generators/gancraft_base.py:588-603): per-pixel feature map
 [N,H,W,64] + style code -> (tanh image, raw image) [N,3,H,W], with RenderCNN.forward (:201-225) evaluated once on the
@@ -15,6 +15,9 @@ from . import _lib
 PRECISION_FP16 = 0      # one fp16 pass per product (the class of the reference's default, cuDNN TF32)
 PRECISION_BF16X3 = 1    # bf16 hi/lo split, 3 passes: the training forward and backward (gradients need bf16's range)
 PRECISION_FP16X3 = 2    # fp16 hi/lo split, 3 passes: fp32-grade (parity default)
+PRECISION_BF16 = 3      # one bf16 pass per product: the training path under bf16 autocast (training only)
+
+TRAIN_PRECISIONS = (PRECISION_FP16, PRECISION_BF16X3, PRECISION_BF16)
 
 _NAMES = ('conv1.weight', 'conv1.bias', 'conv2a.weight', 'conv2a.bias', 'conv2b.weight', 'conv3a.weight', 'conv3a.bias',
           'conv3b.weight', 'conv4a.weight', 'conv4a.bias', 'conv4b.weight', 'conv4b.bias', 'conv4.weight', 'conv4.bias')
@@ -44,30 +47,31 @@ _CONV_W = ('conv1.weight', 'conv2a.weight', 'conv2b.weight', 'conv3a.weight', 'c
 
 
 class _RenderCNNTrainFn(torch.autograd.Function):
-    """(net_out [N,H,W,64], mod [N or 1,4,256], the 14 denoiser tensors in _NAMES order) -> (rgb, raw) [N,3,H,W].
-    The forward packs the weights (bf16 x3) and keeps one record per view; the backward runs sdb_cnn_backward per view
-    and releases the records."""
+    """(precision, net_out [N,H,W,64], mod [N or 1,4,256], the 14 denoiser tensors in _NAMES order) -> (rgb, raw)
+    [N,3,H,W] fp32.  The forward packs the weights at `precision` (one of TRAIN_PRECISIONS) and keeps one record per
+    view; the backward runs sdb_cnn_backward_ex per view at the same precision and releases the records."""
 
     @staticmethod
-    def forward(ctx, net_out, mod, *params):
+    def forward(ctx, precision, net_out, mod, *params):
         L = _lib.lib()
         dev = net_out.device
         N, H, W = net_out.shape[:3]
         x = net_out.detach().contiguous()
         m = mod.detach().to(torch.float32).contiguous()
         ws = [t.detach().to(torch.float32).contiguous() for t in params]
+        ctx.param_dtypes = [t.dtype for t in params]
         rgb = torch.empty(N, 3, H, W, dtype=torch.float32, device=dev)
         raw = torch.empty(N, 3, H, W, dtype=torch.float32, device=dev)
         with torch.cuda.device(dev):
-            pack = torch.empty(int(L.sdb_cnn_pack_bytes(PRECISION_BF16X3)), dtype=torch.uint8, device=dev)
-            _lib.check(L.sdb_cnn_pack(*[_ptr(t) for t in ws], PRECISION_BF16X3, _ptr(pack), _stream(dev)), 'sdb_cnn_pack')
+            pack = torch.empty(int(L.sdb_cnn_pack_bytes_ex(precision)), dtype=torch.uint8, device=dev)
+            _lib.check(L.sdb_cnn_pack_ex(*[_ptr(t) for t in ws], precision, _ptr(pack), _stream(dev)), 'sdb_cnn_pack_ex')
             records = []
             for i in range(N):
-                rec = torch.empty(int(L.sdb_cnn_train_record_bytes(H, W)), dtype=torch.uint8, device=dev)
-                _lib.check(L.sdb_cnn_train_forward(_ptr(x[i]), H, W, _ptr(pack), _ptr(m[i if m.shape[0] > 1 else 0]), _ptr(rgb[i]),
-                                                   _ptr(raw[i]), _ptr(rec), _stream(dev)), 'sdb_cnn_train_forward')
+                rec = torch.empty(int(L.sdb_cnn_train_record_bytes_ex(H, W, precision)), dtype=torch.uint8, device=dev)
+                _lib.check(L.sdb_cnn_train_forward_ex(_ptr(x[i]), H, W, _ptr(pack), _ptr(m[i if m.shape[0] > 1 else 0]), precision,
+                                                      _ptr(rgb[i]), _ptr(raw[i]), _ptr(rec), _stream(dev)), 'sdb_cnn_train_forward_ex')
                 records.append(rec)
-        ctx.records, ctx.pack, ctx.mod, ctx.ws = records, pack, m, ws
+        ctx.records, ctx.pack, ctx.mod, ctx.ws, ctx.precision, ctx.mod_dtype = records, pack, m, ws, precision, mod.dtype
         return rgb, raw
 
     @staticmethod
@@ -76,38 +80,42 @@ class _RenderCNNTrainFn(torch.autograd.Function):
             raise RuntimeError('RenderCNN: the training record of this pass was released by its first backward '
                                '(retain_graph / double backward are not supported on the tensor-core path)')
         L = _lib.lib()
-        records, pack, m, ws = ctx.records, ctx.pack, ctx.mod, ctx.ws
+        records, pack, m, ws, prec = ctx.records, ctx.pack, ctx.mod, ctx.ws, ctx.precision
         ctx.records = None
         dev = pack.device
         N = len(records)
         H, W = (g_rgb if g_rgb is not None else g_raw).shape[2:]
-        need_x, need_m = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
-        need_p = ctx.needs_input_grad[2:]
+        need_x, need_m = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
+        need_p = ctx.needs_input_grad[3:]
         g_rgb = g_rgb.to(torch.float32).contiguous() if g_rgb is not None else None
         g_raw = g_raw.to(torch.float32).contiguous() if g_raw is not None else None
         g_x = torch.empty(N, H, W, 64, dtype=torch.float32, device=dev) if need_x else None
         g_m = torch.empty(N, 4, 256, dtype=torch.float32, device=dev) if need_m else None
         g_p = [torch.zeros_like(w) if need else None for w, need in zip(ws, need_p)]
         with torch.cuda.device(dev):
-            bpack = torch.empty(int(L.sdb_cnn_backward_pack_bytes()), dtype=torch.uint8, device=dev)
+            bpack = torch.empty(int(L.sdb_cnn_backward_pack_bytes_ex(prec)), dtype=torch.uint8, device=dev)
             conv_w = [ws[_NAMES.index(n)] for n in _CONV_W]
-            _lib.check(L.sdb_cnn_pack_backward(*[_ptr(t) for t in conv_w], _ptr(bpack), _stream(dev)), 'sdb_cnn_pack_backward')
-            work = torch.empty(int(L.sdb_cnn_backward_workspace_bytes(H, W)), dtype=torch.uint8, device=dev)
+            _lib.check(L.sdb_cnn_pack_backward_ex(*[_ptr(t) for t in conv_w], prec, _ptr(bpack), _stream(dev)),
+                       'sdb_cnn_pack_backward_ex')
+            work = torch.empty(int(L.sdb_cnn_backward_workspace_bytes_ex(H, W, prec)), dtype=torch.uint8, device=dev)
             view_p = [torch.empty_like(t) if t is not None else None for t in g_p] if N > 1 else g_p
             for i in range(N):
                 grads = _CnnGrads(_ptr(g_x[i]) if need_x else None, _ptr(g_m[i]) if need_m else None,
                                   *[_ptr(t) for t in view_p])
-                _lib.check(L.sdb_cnn_backward(H, W, _ptr(records[i]), _ptr(g_rgb[i]) if g_rgb is not None else None,
-                                              _ptr(g_raw[i]) if g_raw is not None else None, _ptr(bpack), _ptr(pack),
-                                              _ptr(m[i if m.shape[0] > 1 else 0]), ctypes.byref(grads), _ptr(work), _stream(dev)),
-                           'sdb_cnn_backward')
+                _lib.check(L.sdb_cnn_backward_ex(H, W, prec, _ptr(records[i]), _ptr(g_rgb[i]) if g_rgb is not None else None,
+                                                 _ptr(g_raw[i]) if g_raw is not None else None, _ptr(bpack), _ptr(pack),
+                                                 _ptr(m[i if m.shape[0] > 1 else 0]), ctypes.byref(grads), _ptr(work),
+                                                 _stream(dev)), 'sdb_cnn_backward_ex')
                 if N > 1:
                     for acc, v in zip(g_p, view_p):
                         if acc is not None:
                             acc.add_(v)
         if g_m is not None and m.shape[0] == 1 and N > 1:
             g_m = g_m.sum(0, keepdim=True)
-        return (g_x, g_m) + tuple(g_p)
+        if g_m is not None:
+            g_m = g_m.to(ctx.mod_dtype)                          # fc_z_cond(z) is half / bf16 under autocast
+        g_p = [t.to(dt) if t is not None else None for t, dt in zip(g_p, ctx.param_dtypes)]
+        return (None, g_x, g_m) + tuple(g_p)
 
 
 class _CnnGrads(ctypes.Structure):
@@ -146,15 +154,25 @@ class RenderCNNEngine:
         p = self.prefix
         return F.linear(z, self.P[p + 'fc_z_cond.weight'], self.P[p + 'fc_z_cond.bias']).reshape(z.shape[0], 4, 256).contiguous()
 
-    def forward_train(self, net_out, z, P):
+    def forward_train(self, net_out, z, P, precision=PRECISION_BF16X3):
         """Differentiable forward for the training step: P maps the same `denoiser.*` names to the LIVE Parameters
         (state_dict() hands out detached aliases, so self.P cannot carry gradients).  The modulation fc_z_cond(z) is
-        torch's own F.linear, so z, fc_z_cond.weight and .bias get their gradients from autograd."""
+        torch's own F.linear, so z, fc_z_cond.weight and .bias get their gradients from autograd.
+        precision: PRECISION_BF16X3 (fp32-grade), or one pass per product in fp16 (PRECISION_FP16) or bf16
+        (PRECISION_BF16), the class of autocast's own convolutions.  The kernels compute in fp32 at every precision;
+        under autocast rgb and raw are returned in autocast's dtype, as the reference composition returns them there
+        (its convolutions and tanh run in that dtype, gancraft_base.py:201-225, :598-601)."""
         if not net_out.is_cuda or net_out.dtype != torch.float32 or net_out.dim() != 4 or net_out.shape[-1] != 64:
             raise RuntimeError('net_out must be a float32 CUDA tensor [N,H,W,64]')
+        if precision not in TRAIN_PRECISIONS:
+            raise ValueError('RenderCNN training precision must be one of %s, not %r' % (TRAIN_PRECISIONS, precision))
         p = self.prefix
         mod = F.linear(z.to(net_out.device, torch.float32), P[p + 'fc_z_cond.weight'], P[p + 'fc_z_cond.bias'])
-        return _RenderCNNTrainFn.apply(net_out, mod.reshape(z.shape[0], 4, 256), *[P[p + n] for n in _NAMES])
+        rgb, raw = _RenderCNNTrainFn.apply(int(precision), net_out, mod.reshape(z.shape[0], 4, 256), *[P[p + n] for n in _NAMES])
+        if torch.is_autocast_enabled():
+            dt = torch.get_autocast_dtype('cuda')
+            rgb, raw = rgb.to(dt), raw.to(dt)
+        return rgb, raw
 
     def forward(self, net_out, z, want_raw=True):
         """net_out [N,H,W,64] fp32 CUDA, z [N,256] (or [1,256]) -> (fake_images [N,3,H,W], fake_images_raw or None)."""
